@@ -33,6 +33,44 @@ class _Launch:
             _lib.check(rc, self.what)
 
 
+class View:
+    """One tensor a recorded launch reads or writes, as the kernel addresses it (metadata for tests and tools).
+    Layouts: 'nhwc' fp16 [B][h][w][c_stride] (channels c_off .. c_off + c), 'nhwc4b' the fused stem's bordered NHWC4
+    input [B][h + 8][w + 8][4], 'planar8' fp16 chunk-planar [B][c / 8][h][w][8] (fm_osb_streams tails), 'gap_part' fp32
+    [B][strips][4][c] per-strip channel sums, 'f32' fp32 vectors [B][c]."""
+    __slots__ = ("name", "t", "layout", "c", "h", "w", "c_stride", "c_off", "strips")
+
+    def __init__(self, name, t, layout, c, h=1, w=1, c_stride=None, c_off=0, strips=None):
+        self.name, self.t, self.layout, self.c, self.h, self.w = name, t, layout, c, h, w
+        self.c_stride = c if c_stride is None else c_stride
+        self.c_off, self.strips = c_off, strips
+
+    def array(self, n):
+        """The first n rows of the batch, shaped by the layout (a view into the buffer, not a copy)."""
+        t, c, h, w = self.t.reshape(-1), self.c, self.h, self.w
+        if self.layout == 'nhwc':
+            return t[:n * h * w * self.c_stride].view(n, h, w, self.c_stride)[..., self.c_off:self.c_off + c]
+        if self.layout == 'nhwc4b':
+            return t[:n * (h + 8) * (w + 8) * 4].view(n, h + 8, w + 8, 4)
+        if self.layout == 'planar8':
+            return t[:n * h * w * c].view(n, c // 8, h, w, 8)
+        if self.layout == 'gap_part':
+            return t[:n * self.strips * 4 * c].view(n, self.strips, 4, c)
+        if self.layout == 'f32':
+            return t[:n * c].view(n, c)
+        raise ValueError(self.layout)
+
+
+class TraceEntry:
+    """What one recorded launch computes: `kind` ('stem', 'S' = fm_osb_streams, 'G' = fm_osb_merge, 'conv', 'conv+add'
+    = conv with the residual add + ReLU in its epilogue, 'gate4_pooled', or the op kind of models/osnet.py), the
+    indices of the ops it implements, and the views it reads and writes."""
+    __slots__ = ("kind", "ops", "ins", "outs")
+
+    def __init__(self, kind, ops, ins, outs):
+        self.kind, self.ops, self.ins, self.outs = kind, tuple(ops), list(ins), list(outs)
+
+
 def _conv_desc(n, hi, wi, cin, cin_stride, cin_off, ho, wo, cout, cout_stride, cout_off, k, stride, pad, act, ws=None):
     d = _lib.FmConvDesc()
     if ws is not None:       # fp32 split-K scratch (a torch uint8 tensor owned by the caller)
@@ -337,6 +375,20 @@ class OSNetEngine(_Net):
                 params[name] = tuple(torch.as_tensor(a).to(dev) for a in self.weights[name])
             return params[name]
 
+        # self.trace[i] describes self.launches[i] (TraceEntry): which ops it implements, the views it reads and writes
+        self.trace = []
+        views = {'input': View('input', self.inp, 'nhwc4b', 4, H, W) if self.fuse_stem
+                 else View('input', self.inp, 'nhwc', IN_C_PAD, H, W)}
+
+        def nhwc(name):
+            """The NHWC view of a live buffer, recorded under its name."""
+            t_, c_, h_, w_ = live[name]
+            views[name] = View(name, t_, 'nhwc', c_, h_, w_)
+            return views[name]
+
+        def trace(kind, ks, ins, outs):
+            self.trace.append(TraceEntry(kind, ks, [views[s_] for s_ in ins], outs))
+
         self.pooled = torch.zeros(4 * B, 512, dtype=torch.float32, device=dev)
         self.gate_tmp = torch.zeros(4 * B, 512, dtype=torch.float32, device=dev)
         self._params = params
@@ -361,6 +413,7 @@ class OSNetEngine(_Net):
                 self.n_tc += 1
                 self.layer_bytes += 2 * (B * (H + 8) * (W + 8) * 4 + B * 64 * 32 * 64)
                 live[self.ops[1][2]] = (y, 64, 64, 32)
+                trace('stem', (0, 1), ['input'], [nhwc(self.ops[1][2])])
                 skip_until = 1
                 continue
             if kind == 'conv' and self.fuse_osb and op[4] == 1 and op[7] == 'relu':     # OSBlock candidate (structural)
@@ -402,7 +455,11 @@ class OSNetEngine(_Net):
                     self.layer_bytes += 2 * (B * h * w * (xc + 4 * mid))
                     for i, tn in enumerate(tails_names):
                         live[tn] = (tails[i], mid, h, w)
+                        views[tn] = View(tn, tails[i], 'planar8', mid, h, w)
                     pooled_by_tail[tails_names[0]] = (gap, strips)
+                    gname = tails_names[0] + '.gap'
+                    views[gname] = View(gname, gap, 'gap_part', mid, h, w, strips=strips)
+                    trace('S', range(k, gate_k), [op[8]], [views[tn] for tn in tails_names] + [views[gname]])
                     # the block input may die here (no identity / downsample use): same bookkeeping as below
                     for name in self._reads(op):
                         if last.get(name) == k:
@@ -429,10 +486,12 @@ class OSNetEngine(_Net):
                     self._conv(d, x, wd, bd, y, residual=live[nxt[2]][0])
                     fused_add[k + 1] = nxt[2]
                     new = (nxt[3], (y, cout, ho, wo))
+                    trace('conv+add', (k, k + 1), [src, nxt[2]], [View(new[0], new[1][0], 'nhwc', *new[1][1:])])
                 else:
                     d = _conv_desc(B, h, w, xc, xc, 0, ho, wo, cout, cout, 0, ks, stride, pad, _ACT[act])
                     self._conv(d, x, wd, bd, y)
                     new = (dst, (y, cout, ho, wo))
+                    trace('conv', (k,), [src], [View(new[0], new[1][0], 'nhwc', *new[1][1:])])
             elif kind == 'dw':
                 _, name, c, act, src, dst = op
                 x, xc, h, w = live[src]
@@ -443,17 +502,20 @@ class OSNetEngine(_Net):
                 self._add('fm_dwconv3', ptr(x), ptr(wd), ptr(bd), ptr(y), B, h, w, c, _ACT[act])
                 self.layer_bytes += 2 * (2 * B * h * w * c + 9 * c)
                 new = (dst, (y, c, h, w))
+                trace(kind, (k,), [src], [View(new[0], new[1][0], 'nhwc', *new[1][1:])])
             elif kind == 'maxpool3s2':
                 x, xc, h, w = live[op[1]]
                 ho, wo = (h + 2 - 3) // 2 + 1, (w + 2 - 3) // 2 + 1
                 y = alloc(B * ho * wo * xc)
                 self._add('fm_maxpool_pad', ptr(x), ptr(y), B, h, w, xc, 3, 2, 1)
                 new = (op[2], (y, xc, ho, wo))
+                trace(kind, (k,), [op[1]], [View(new[0], new[1][0], 'nhwc', *new[1][1:])])
             elif kind == 'avgpool2':
                 x, xc, h, w = live[op[1]]
                 y = alloc(B * (h // 2) * (w // 2) * xc)
                 self._add('fm_avgpool2', ptr(x), ptr(y), B, h, w, xc)
                 new = (op[2], (y, xc, h // 2, w // 2))
+                trace(kind, (k,), [op[1]], [View(new[0], new[1][0], 'nhwc', *new[1][1:])])
             elif kind == 'gate':
                 _, name, c, src, acc, accumulate = op
                 x, xc, h, w = live[src]
@@ -463,6 +525,7 @@ class OSNetEngine(_Net):
                 a = live[acc][0]
                 self._add('fm_channel_gate', ptr(x), ptr(self.pooled), ptr(self.gate_tmp), ptr(w1), ptr(b1), ptr(w2),
                           ptr(b2), ptr(a), B, h * w, c, w1.shape[0], accumulate)
+                trace(kind, (k,), [src, acc] if accumulate else [src], [nhwc(acc)])
                 new = None
             elif kind == 'gate4' and op[3][0] in pooled_by_tail and self._match_merge(k) is not None and \
                     self._lib.fm_osb_merge_ncta(op[2], self._match_merge(k)[1][3]) > 0:
@@ -514,6 +577,8 @@ class OSNetEngine(_Net):
                 if add_op[3] in live:
                     release(add_op[3])
                 live[add_op[3]] = (y, cout, h, w)
+                trace('G', range(k, last_k + 1), list(srcs) + [srcs[0] + '.gap', ds_op[8] if ds_op else ident_name],
+                      [nhwc(add_op[3])])
                 skip_until = last_k
                 continue
             elif kind == 'gate4':
@@ -527,10 +592,12 @@ class OSNetEngine(_Net):
                     self._add('fm_channel_gate4_pooled', ptr(xs[0]), ptr(xs[1]), ptr(xs[2]), ptr(xs[3]), ptr(gap),
                               strips, ptr(self.gate_tmp), ptr(w1), ptr(b1), ptr(w2), ptr(b2), ptr(a), B, h * w, c,
                               w1.shape[0])
+                    trace('gate4_pooled', (k,), list(srcs) + [srcs[0] + '.gap'], [View(acc, a, 'nhwc', c, h, w)])
                 else:
                     self._add('fm_channel_gate4', ptr(xs[0]), ptr(xs[1]), ptr(xs[2]), ptr(xs[3]), ptr(self.pooled),
                               ptr(self.gate_tmp), ptr(w1), ptr(b1), ptr(w2), ptr(b2), ptr(a), B, h * w, c,
                               w1.shape[0])
+                    trace(kind, (k,), list(srcs), [View(acc, a, 'nhwc', c, h, w)])
                 new = (acc, (a, c, h, w))
             elif kind == 'add_relu':
                 if k in fused_add:        # folded into the preceding conv's epilogue
@@ -540,16 +607,19 @@ class OSNetEngine(_Net):
                 y = alloc(B * h * w * ac)
                 self._add('fm_add_act', ptr(a), ptr(b), ptr(y), B * h * w * ac, _ACT['relu'])
                 new = (op[3], (y, ac, h, w))
+                trace(kind, (k,), [op[1], op[2]], [View(new[0], new[1][0], 'nhwc', *new[1][1:])])
             elif kind == 'gap':
                 x, xc, h, w = live[op[1]]
                 y = alloc(B * xc, torch.float32)
                 self._add('fm_global_avgpool', ptr(x), ptr(y), B, h * w, xc)
                 new = (op[2], (y, xc, 1, 1))
+                trace(kind, (k,), [op[1]], [View(op[2], y, 'f32', xc)])
             elif kind == 'fc':
                 _, name, cin, cout, src, dst = op
                 x = live[src][0]
                 wd, bd = dparam(name)
                 self._add('fm_fc_norm', ptr(x), ptr(wd), ptr(bd), ptr(self.out), B, cin, cout, 1, 1)
+                trace(kind, (k,), [src], [View(dst, self.out, 'f32', cout)])
                 new = None
             else:
                 raise NotImplementedError(kind)
@@ -560,6 +630,7 @@ class OSNetEngine(_Net):
                 if new[0] in live:
                     release(new[0])
                 live[new[0]] = new[1]
+                views[new[0]] = self.trace[-1].outs[0]
 
     def _match_osblock(self, k):
         """ops[k] = '<blk>.conv1'; returns (tail buffer names of the four streams, index of the gate4 op) when the next

@@ -29,14 +29,17 @@ CONV_CASES = [
 
 
 def _run_conv(fn_name, case, seed=0):
+    """case: the CONV_CASES fields, optionally followed by res_first: FM_ACT_AFTER_RESIDUAL, act(conv + b + res)
+    instead of the Darknet order act(conv + b) + res."""
     from fastmot_b200 import _lib
     from fastmot_b200.devmem import ptr, stream_ptr
-    from fastmot_b200.engine import _conv_desc
+    from fastmot_b200.engine import ACT_AFTER_RESIDUAL, _conv_desc
     from fastmot_b200.models.darknet import ACTS
     from oracle.nets import _act
     lib = _lib.load()
     ws = torch.empty(32 << 20, dtype=torch.uint8, device="cuda")   # enables split-K for small-M / large-K shapes
-    n, h, w, cin, cout, k, stride, act, cis, cio, cos, coo, use_res = case
+    n, h, w, cin, cout, k, stride, act, cis, cio, cos, coo, use_res = case[:13]
+    res_first = len(case) > 13 and case[13]
     g = torch.Generator().manual_seed(seed)
     pad = k // 2
     ho, wo = (h + 2 * pad - k) // stride + 1, (w + 2 * pad - k) // stride + 1
@@ -45,7 +48,8 @@ def _run_conv(fn_name, case, seed=0):
     bias = torch.randn(cout, generator=g) * 0.1
     res = (torch.randn(n, ho, wo, cout, generator=g) * 0.5).half() if use_res else None
     out = torch.zeros(n, ho, wo, cos, dtype=torch.float16)
-    d = _conv_desc(n, h, w, cin, cis, cio, ho, wo, cout, cos, coo, k, stride, pad, ACTS[act], ws=ws)
+    d = _conv_desc(n, h, w, cin, cis, cio, ho, wo, cout, cos, coo, k, stride, pad,
+                   ACTS[act] | (ACT_AFTER_RESIDUAL if res_first else 0), ws=ws)
     if use_res:
         d.res_stride, d.res_offset = cout, 0
     if fn_name == 'fm_conv2d_tc' and not lib.fm_conv2d_tc_supported(C.byref(d)):
@@ -60,9 +64,12 @@ def _run_conv(fn_name, case, seed=0):
     got = od.cpu().float()
     xs = xin[..., cio:cio + cin].float().permute(0, 3, 1, 2)
     y = F.conv2d(xs, wt.float().permute(0, 3, 1, 2), bias, stride=stride, padding=pad)
-    y = _act(y, act)
-    if use_res:
-        y = y + res.float().permute(0, 3, 1, 2)
+    if res_first:
+        y = _act(y + res.float().permute(0, 3, 1, 2), act)
+    else:
+        y = _act(y, act)
+        if use_res:
+            y = y + res.float().permute(0, 3, 1, 2)
     want = y.permute(0, 2, 3, 1)
     assert _rel(got[..., coo:coo + cout], want) < 4e-3, (fn_name, case, _rel(got[..., coo:coo + cout], want))
     untouched = torch.cat([got[..., :coo], got[..., coo + cout:]], -1)
@@ -70,9 +77,31 @@ def _run_conv(fn_name, case, seed=0):
     return True
 
 
-@pytest.mark.parametrize("case", CONV_CASES)
+# FM_ACT_AFTER_RESIDUAL (res_first, last field): out = act(conv + b + res), the order of OSNet's conv3 + add + ReLU
+RES_FIRST_SIMT = [
+    (1, 24, 24, 64, 64, 3, 1, 'leaky', 64, 0, 64, 0, True, True),
+    (2, 16, 8, 40, 20, 1, 1, 'relu', 40, 0, 20, 0, True, True),
+]
+
+
+@pytest.mark.parametrize("case", CONV_CASES + RES_FIRST_SIMT)
 def test_conv_simt_vs_torch(case):
     assert _run_conv('fm_conv2d_simt', case)
+
+
+# every epilogue branch of conv_tc.cu with FM_ACT_AFTER_RESIDUAL (shapes chosen from fm_conv2d_tc / launch_tc)
+RES_FIRST_TC = [
+    (2, 16, 8, 96, 384, 1, 1, 'relu', 96, 0, 384, 0, True, True),      # nk 2, no split, 8-aligned: epilogue_staged
+    (1, 12, 12, 64, 36, 1, 1, 'leaky', 64, 0, 48, 0, True, True),      # cout 36: epilogue_store32, 16-aligned stores
+    (1, 12, 12, 64, 36, 1, 1, 'leaky', 64, 0, 40, 0, True, True),      # stride 40: epilogue_store32 element-wise
+    (1, 10, 10, 512, 64, 3, 1, 'leaky', 512, 0, 64, 0, True, True),    # 1 tile, nk 72: split-K, 8-wide reduce
+    (1, 10, 10, 640, 20, 1, 1, 'leaky', 640, 0, 20, 0, True, True),    # 1 tile, nk 10, cout 20: scalar reduce
+]
+
+
+@pytest.mark.parametrize("case", RES_FIRST_TC)
+def test_conv_tc_act_after_residual(case):
+    assert _run_conv('fm_conv2d_tc', case)
 
 
 @pytest.mark.parametrize("case", CONV_CASES + [
@@ -125,7 +154,16 @@ TMA_CASES = [
 ]
 
 
-@pytest.mark.parametrize("case", TMA_CASES)
+# conv_tma.cu epilogue with FM_ACT_AFTER_RESIDUAL; plans from fm_conv2d_tma / pick_split (FM_CONV_TMA_VERBOSE=1)
+RES_FIRST_TMA = [
+    (4, 64, 32, 128, 128, 1, 1, 'leaky', 128, 0, 128, 0, True, True),  # 64-wide, 128 tiles, nk 2: S == 1, vector
+    (1, 20, 20, 512, 256, 3, 1, 'leaky', 512, 0, 256, 0, True, True),  # 4 x 2 tiles, nk 72: S > 1, vector
+    (1, 26, 26, 64, 36, 1, 1, 'leaky', 64, 0, 36, 0, True, True),      # cout 36, nk 1: S == 1, element-wise
+    (1, 20, 20, 1024, 18, 1, 1, 'leaky', 1024, 0, 18, 0, True, True),  # cout 18, 4 tiles, nk 16: S > 1, element-wise
+]
+
+
+@pytest.mark.parametrize("case", TMA_CASES + RES_FIRST_TMA)
 def test_conv_tma_vs_torch(case):
     """TMA-fed wgmma conv with in-cluster split-K (csrc/conv_tma.cu) vs fp32 torch."""
     assert _run_conv('fm_conv2d_tma', case)

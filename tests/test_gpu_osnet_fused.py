@@ -17,22 +17,11 @@ def _h(t):
 
 
 def _streams_reference(x, w1, b1, pws, dws):
-    """x: (n, h, w, cin) fp32 (already fp16-representable).  Returns 4 tails (n, h, w, mid) and their channel sums."""
-    xc = x.permute(0, 3, 1, 2)
-    mid = w1.shape[0]
-    x1 = _h(F.relu(F.conv2d(xc, _h(w1)[:, :, None, None], b1)))
-    tails = []
-    lvl = 0
-    for s in range(4):
-        cur = x1
-        for _ in range(s + 1):
-            wp, bp = pws[lvl]
-            wd, bd = dws[lvl]
-            p = _h(F.conv2d(cur, _h(wp)[:, :, None, None], bp))
-            k = _h(wd).reshape(3, 3, mid).permute(2, 0, 1).unsqueeze(1).contiguous()
-            cur = _h(F.relu(F.conv2d(p, k, _h(bd), padding=1, groups=mid)))
-            lvl += 1
-        tails.append(cur.permute(0, 2, 3, 1).contiguous())
+    """x: (n, h, w, cin) fp32 (already fp16-representable).  Returns 4 tails (n, h, w, mid) and their channel sums
+    (the float64 reference of kernel S, oracle/nets64.py, with fp16 weights as the kernel reads them)."""
+    from oracle import nets64
+    tails = nets64.osb_streams(x, _h(w1), b1, [(_h(w), b) for w, b in pws], [(_h(w), b) for w, b in dws])
+    tails = [t.float() for t, _ in tails]
     return tails, [t.sum((1, 2)) for t in tails]
 
 
@@ -212,16 +201,17 @@ def test_osb_merge_vs_torch(w, mid, h, cin, cout, n):
     else:
         res = (torch.randn(n, h * w, cout, generator=g).abs() * 0.7).half()
         got = run_osb_merge([t.cuda() for t in tails], gw, w3, b3, res=res.cuda())
+    from oracle import nets64
     t = lambda a: torch.as_tensor(np.asarray(a, np.float32))
-    u = 0
-    for s in range(4):
-        tf = tails[s].float()
-        gate = torch.sigmoid(F.relu(tf.mean((1, 2)) @ t(gw[0]).T + t(gw[1])) @ t(gw[2]).T + t(gw[3]))
-        u = u + tf * gate[:, None, None, :]
-    u = _h(u).reshape(n, h * w, mid)
-    y = u @ _h(t(w3)).T + t(b3)
-    y = y + (x.float() @ _h(t(wd)).T + t(bd) if down else res.float())
-    want = _h(F.relu(y))
+    gap = torch.stack([torch.stack([tl.float()[:, :h // 2].sum((1, 2)), tl.float()[:, h // 2:].sum((1, 2))], 1)
+                       for tl in tails], 2)                        # the strip sums run_osb_merge hands the kernel
+    gwt = tuple(t(a) for a in gw)
+    if down:
+        want, _ = nets64.osb_merge(tails, gap, gwt, _h(t(w3)), t(t(b3) + t(bd)), x=x.reshape(n, h, w, cin),
+                                   wd=_h(t(wd)))
+    else:
+        want, _ = nets64.osb_merge(tails, gap, gwt, _h(t(w3)), t(b3), res=res.reshape(n, h, w, cout))
+    want = want.float().reshape(n, h * w, cout)
     gotc = got.float().cpu()
     assert torch.isfinite(gotc).all()
     err = float((gotc - want).abs().max()) / (float(want.abs().max()) + 1e-6)
