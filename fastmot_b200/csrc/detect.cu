@@ -71,13 +71,14 @@ __global__ void yolo_decode_filter_kernel(const T* __restrict__ in, int yolo_w, 
     if (!label_mask[class_id]) return;
     const float score = __fmul_rn(box_prob, cls_prob);
     if (!((double)score >= conf_thresh)) return;
-    // detector.py:339-341: scale to pixels (f32 <- f64 product), subtract letterbox offset
-    float px = (float)((double)bx * (double)size_w);
-    float py = (float)((double)by * (double)size_h);
-    float pw = (float)((double)bw * (double)size_w);
-    float ph = (float)((double)bh * (double)size_h);
-    px = (float)((double)px - (double)off_x);
-    py = (float)((double)py - (double)off_y);
+    // detector.py:339-341: scale to pixels (f32 <- f64 product), subtract letterbox offset.  The f64 product of two
+    // floats is exact, so its f32 rounding is __fmul_rn; likewise the f32 rounding of the f64 difference is __fsub_rn.
+    // Written as f64 casts the compiler lowered both to plain mul.f32 / sub.f32, which ptxas contracted into one FFMA:
+    // the product was never rounded and py differed from the reference by up to half an ulp of by * size_h.
+    const float px = __fsub_rn(__fmul_rn(bx, size_w), off_x);
+    const float py = __fsub_rn(__fmul_rn(by, size_h), off_y);
+    const float pw = __fmul_rn(bw, size_w);
+    const float ph = __fmul_rn(bh, size_h);
     const int gidx = cand_base + idx;
     float* d = dense + (size_t)gidx * 8;
     d[0] = px; d[1] = py; d[2] = pw; d[3] = ph; d[4] = box_prob; d[5] = (float)class_id; d[6] = cls_prob;

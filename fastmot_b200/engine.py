@@ -63,12 +63,15 @@ class View:
 
 class TraceEntry:
     """What one recorded launch computes: `kind` ('stem', 'S' = fm_osb_streams, 'G' = fm_osb_merge, 'conv', 'conv+add'
-    = conv with the residual add + ReLU in its epilogue, 'gate4_pooled', or the op kind of models/osnet.py), the
-    indices of the ops it implements, and the views it reads and writes."""
-    __slots__ = ("kind", "ops", "ins", "outs")
+    = conv with the residual add + ReLU in its epilogue, 'gate4_pooled', or the op kind of models/osnet.py; for the
+    detector 'conv', 'conv+shortcut', 'maxpool', 'upsample', 'copy', 'shortcut'), the indices of the ops (Darknet
+    layers) it implements, the views it reads and writes, and kind-specific details in `info` (the conv path, the
+    window a max-pool launches)."""
+    __slots__ = ("kind", "ops", "ins", "outs", "info")
 
-    def __init__(self, kind, ops, ins, outs):
+    def __init__(self, kind, ops, ins, outs, info=None):
         self.kind, self.ops, self.ins, self.outs = kind, tuple(ops), list(ins), list(outs)
+        self.info = dict(info or {})
 
 
 def _conv_desc(n, hi, wi, cin, cin_stride, cin_off, ho, wo, cout, cout_stride, cout_off, k, stride, pad, act, ws=None):
@@ -102,22 +105,24 @@ class _Net:
         self.ws = torch.empty(self.WS_BYTES, dtype=torch.uint8, device=self.dev)
 
     def _conv(self, desc, x, w, b, out, residual=None):
+        """Records the conv on the path that supports it; returns that path: 'tma', 'tc' or 'simt'."""
         lib = self._lib
         desc.ws, desc.ws_bytes = self.ws.data_ptr(), self.ws.numel()
         self._keep.append(desc)
         self.layer_bytes += 2 * (desc.n * desc.hi * desc.wi * desc.cin + desc.n * desc.ho * desc.wo * desc.cout
                                  * (2 if residual is not None else 1) + desc.kh * desc.kw * desc.cin * desc.cout)
         if self.use_tc and self.use_tma and lib.fm_conv2d_tma_supported(C.byref(desc)):
-            fn = lib.fm_conv2d_tma          # TMA-fed, cluster split-K (csrc/conv_tma.cu)
+            fn, path = lib.fm_conv2d_tma, 'tma'         # TMA-fed, cluster split-K (csrc/conv_tma.cu)
             self.n_tc += 1
             self.n_tma += 1
         elif self.use_tc and lib.fm_conv2d_tc_supported(C.byref(desc)):
-            fn = lib.fm_conv2d_tc
+            fn, path = lib.fm_conv2d_tc, 'tc'
             self.n_tc += 1
         else:
-            fn = lib.fm_conv2d_simt
+            fn, path = lib.fm_conv2d_simt, 'simt'
             self.n_simt += 1
         self.launches.append(_Launch(fn, (C.byref(desc), ptr(x), ptr(w), ptr(b), ptr(residual), ptr(out)), "conv"))
+        return path
 
     def kernels_per_replay(self):
         extra = {'fm_channel_gate': 2, 'fm_channel_gate4': 2, 'fm_channel_gate4_pooled': 1, 'fm_osb_merge': 1}
@@ -206,6 +211,15 @@ class YoloEngine(_Net):
                     nx.get('activation', 'linear') == 'linear' and not refs.get(i) and nx['from_abs'] < i and \
                     self.shapes[nx['from_abs']] == self.shapes[i]:
                 self.fused_shortcuts.add(i + 1)
+        # self.trace[k] describes self.launches[k] (TraceEntry): the layers it implements, the views it reads and writes
+        self.trace = []
+
+        def vw(j, v=None):
+            """The View of layer j's output (j = -1: the network input), or of the view tuple v named after j."""
+            t_, c_, cs_, co_, h_, w_ = v if v is not None else (self.views[j] if j >= 0 else
+                                                                (self.inp, IN_C_PAD, IN_C_PAD, 0, H, W))
+            return View('input' if j < 0 else f"L{j}", t_, 'nhwc', c_, h_, w_, cs_, co_)
+
         spp_prev = {}
         for i, l in enumerate(L):
             t = l['type']
@@ -231,32 +245,42 @@ class YoloEngine(_Net):
                 d = _conv_desc(1, src[4], src[5], cin, src[2], src[3], h, w, c, out[2], out[3], k, l.get('stride', 1),
                                pad, _ACT[l.get('activation', 'linear')])
                 if i + 1 in self.fused_shortcuts:
-                    b = self.views[L[i + 1]['from_abs']]
+                    fr = L[i + 1]['from_abs']
+                    b = self.views[fr]
                     d.res_stride, d.res_offset = b[2], b[3]
-                    self._conv(d, src[0], wd, bd, out[0], residual=b[0])
+                    path = self._conv(d, src[0], wd, bd, out[0], residual=b[0])
+                    self.trace.append(TraceEntry('conv+shortcut', (i, i + 1), [vw(i - 1), vw(fr)], [vw(i, out)],
+                                                 {'path': path}))
                 else:
-                    self._conv(d, src[0], wd, bd, out[0])
+                    path = self._conv(d, src[0], wd, bd, out[0])
+                    self.trace.append(TraceEntry('conv', (i,), [vw(i - 1)], [vw(i, out)], {'path': path}))
             elif t == 'maxpool':
-                ksz, psrc = l['size'], src
+                ksz, psrc, pj = l['size'], src, i - 1
                 key = (src[0].data_ptr(), src[1], src[2], src[3])
                 if l['stride'] == 1 and ksz % 2 == 1:
                     # SPP (5 / 9 / 13 on the same tensor): a k x k stride-1 max over a k0 x k0 max is the
                     # (k + k0 - 1) window, so 9 = 5 o 5 and 13 = 5 o 9 -- each pool reads 25 taps instead of 81 / 169
                     prev = spp_prev.get(key)
                     if prev is not None and ksz > prev[0]:
-                        ksz, psrc = ksz - prev[0] + 1, prev[1]
-                    spp_prev[key] = (l['size'], out)
+                        ksz, psrc, pj = ksz - prev[0] + 1, prev[1], prev[2]
+                    spp_prev[key] = (l['size'], out, i)
                 self._add('fm_maxpool', ptr(psrc[0]), ptr(out[0]), 1, psrc[4], psrc[5], psrc[1], psrc[2], psrc[3],
                           ksz, l['stride'], out[2], out[3])
+                # ins[0] is the declared source; a composed SPP pool also reads the smaller pool's output
+                self.trace.append(TraceEntry('maxpool', (i,), [vw(i - 1)] + ([vw(pj)] if pj != i - 1 else []),
+                                             [vw(i, out)], {'size': l['size'], 'src': i - 1, 'stride': l['stride'],
+                                                            'launch_size': ksz, 'launch_src': pj}))
             elif t == 'upsample':
                 self._add('fm_upsample_copy', ptr(src[0]), ptr(out[0]), 1, src[4], src[5], src[1], src[2], src[3],
                           l['stride'], out[2], out[3])
+                self.trace.append(TraceEntry('upsample', (i,), [vw(i - 1)], [vw(i, out)], {'stride': l['stride']}))
             elif t == 'shortcut' and i in self.fused_shortcuts:
                 out = self.views[i - 1]          # already holds conv + residual
             elif t == 'shortcut':
                 a, b = self.views[i - 1], self.views[l['from_abs']]
                 self._add('fm_add_act_strided', ptr(a[0]), a[2], a[3], ptr(b[0]), b[2], b[3], ptr(out[0]), out[2],
                           out[3], h * w, c, _ACT[l.get('activation', 'linear')])
+                self.trace.append(TraceEntry('shortcut', (i,), [vw(i - 1), vw(l['from_abs'])], [vw(i, out)]))
             elif t == 'route':
                 srcs = l['layers_abs']
                 g = l.get('groups', 1)
@@ -273,6 +297,9 @@ class YoloEngine(_Net):
                         if home.get(s, (None,))[0] != i:
                             self._add('fm_upsample_copy', ptr(sv[0]), ptr(buf), 1, sv[4], sv[5], cs, sv[2],
                                       sv[3] + l.get('group_id', 0) * cs, 1, c, off)
+                            self.trace.append(TraceEntry(
+                                'copy', (i,), [vw(s, (sv[0], cs, sv[2], sv[3] + l.get('group_id', 0) * cs) + sv[4:])],
+                                [vw(i, (buf, cs, c, off, h, w))], {'src': s}))
                         off += cs
                     out = (buf, c, c, 0, h, w)
             elif t == 'yolo':

@@ -1,6 +1,7 @@
 """TEST INFRASTRUCTURE ONLY.  float64 reference of every OSNet op (models/osnet.py vocabulary) and of the fused units
-the engine launches (the stem, fm_osb_streams = "S", fm_osb_merge = "G"), each with a per-element error bound
-derived from the rounding model of the kernel that computes it.
+the engine launches (the stem, fm_osb_streams = "S", fm_osb_merge = "G"), of the Darknet layers the detector engine
+launches (conv with every activation, max-pool, upsample, route copy, shortcut) and of the head decode, each with a
+per-element error bound derived from the rounding model of the kernel that computes it.
 
 Every function takes the fp16 / fp32 values the kernel read (any torch dtype, any device; NHWC activations) and
 returns (want, bound) as float64 tensors: `want` is the exact result rounded to fp16 wherever the kernel stores
@@ -14,6 +15,8 @@ import math
 
 import torch
 import torch.nn.functional as F
+
+from fastmot_b200.models import darknet
 
 U16 = 2.0 ** -11
 U32 = 2.0 ** -24
@@ -47,15 +50,67 @@ def _nhwc(x):
 
 
 def _act(v, act):
-    return v.clamp_min(0) if act == 'relu' else v
+    """The activations of csrc/conv_act.cuh and nn.cu (Darknet semantics), exact."""
+    if act == 'linear':
+        return v
+    if act == 'relu':
+        return v.clamp_min(0)
+    if act == 'leaky':
+        return torch.where(v > 0, v, 0.1 * v)
+    if act == 'logistic':
+        return torch.sigmoid(v)
+    if act == 'swish':
+        return v * torch.sigmoid(v)
+    if act == 'mish':
+        return v * torch.tanh(F.softplus(v))
+    raise ValueError(act)
+
+
+def _expf_rel(x):
+    """Relative error of __expf(x) (ex2.approx and the fp32 product x log2(e)), as in gate_vector."""
+    return 2.0 ** -21 + x.abs() * 2.0 ** -23
+
+
+def _act_bound(v, e, act):
+    """(act(v), bound) for a kernel that holds the pre-activation as v_k, |v_k - v| <= e, and applies the fp32
+    activation of conv_act.cuh / nn.cu to it.  The bound is the largest slope of the activation on [v - e, v + e]
+    times e, plus the activation's own rounding relative to |act(v)|:
+      linear 0; relu 0 (slope 0 where v + e <= 0);
+      leaky   slope 0.1 where v + e <= 0; the product 0.1f * v: the constant 0.1f (off by 1.5e-8 relative) and
+              one rounding, 2 u32;
+      logistic 1 / (1 + __expf(-v)): slope <= 1/4; the relative error d of __expf(-v) reaches 1 / (1 + n) damped
+              by n / (1 + n) <= 1; the add and the (IEEE or __fdividef 2-ulp) division: d + 4 u32;
+      swish   v / (1 + __expf(-v)): slope <= 1.1 (max 1.0998 at v ~ 2.4); d + 4 u32;
+      mish    v r, r = t / (t + 2), t = n (n + 2), n = __expf(min(v, 20)): slope <= 1.1 (max 1.089 at v ~ 1.2);
+              d ln r / d ln n <= 1, so r inherits the relative error d of n; t (2 roundings), t + 2, __fdividef
+              (2 ulp) and the product by v add 8 u32.  The clamp at v = 20 changes r by < 1e-16 relative.  nn.cu's
+              SIMT form v tanh(log1p(n)) is the same function of n (log1pf 1 ulp, tanhf 2 ulp, both damped by
+              slopes <= 1 in the log domain) and is inside the same bound.
+    d is taken at |v| + e: the kernel's argument is v_k, not v."""
+    y = _act(v, act)
+    if act == 'linear':
+        return y, e
+    if act == 'relu':
+        return y, torch.where(v + e > 0, e, torch.zeros_like(e))
+    if act == 'leaky':
+        return y, torch.where(v + e > 0, e, 0.1 * e) + 2 * U32 * y.abs()
+    if act == 'logistic':
+        return y, 0.25 * e + y.abs() * (_expf_rel(v.abs() + e) + 4 * U32)
+    if act == 'swish':
+        return y, 1.1 * e + y.abs() * (_expf_rel(v.abs() + e) + 4 * U32)
+    if act == 'mish':
+        return y, 1.1 * e + y.abs() * (_expf_rel((v.abs() + e).clamp_max(20.0)) + 8 * U32)
+    raise ValueError(act)
 
 
 # ------------------------------------------------------------------------------------------------- single ops
 def conv(x, w, b, stride=1, pad=0, act='linear', res=None, res_first=True, q=True):
     """Dense conv, NHWC: x (n, h, w, cin), w (cout, k, k, cin), b (cout), optional residual (n, ho, wo, cout).
-    act(conv + b + res) when res_first (FM_ACT_AFTER_RESIDUAL, OSNet conv3), else act(conv + b) + res.
+    act(conv + b + res) when res_first (FM_ACT_AFTER_RESIDUAL, OSNet conv3), else act(conv + b) + res (the Darknet
+    order of a shortcut fused into the conv's epilogue).
     Model (wgmma or SIMT, fp32 accumulation, fp16 store):
-        u |acc| + K u32 S|xw| + 3 u32 (|acc| + |b| + |res|), then the fp16 store (_store16).
+        pre-activation u |acc| + K u32 S|xw| + 3 u32 (|acc| + |b| + |res|), through the activation (_act_bound),
+        + u32 |out| for a residual added after it, then the fp16 store (_store16).
     `acc` is the pre-bias sum: the staged epilogue rounds it to fp16 before adding the bias (conv_tc.cu
     epilogue_staged, conv_tma.cu S == 1); the other epilogues add in fp32, for which the term is merely loose."""
     x, w, b = _d(x), _d(w), _d(b)
@@ -64,10 +119,16 @@ def conv(x, w, b, stride=1, pad=0, act='linear', res=None, res_first=True, q=Tru
     acc = _nhwc(F.conv2d(_nchw(x), wt, None, stride=stride, padding=pad))
     sabs = _nhwc(F.conv2d(_nchw(x.abs()), wt.abs(), None, stride=stride, padding=pad))
     r = torch.zeros_like(acc) if res is None else _d(res)
-    v = acc + b
-    v = _act(v + r, act) if res_first else _act(v, act) + r
     kk = k * k * x.shape[-1]
     e = U16 * acc.abs() + kk * U32 * sabs + 3 * U32 * (acc.abs() + b.abs() + r.abs())
+    v = acc + b
+    if res_first:
+        v, e = _act_bound(v + r, e, act)
+    else:
+        v, e = _act_bound(v, e, act)
+        if res is not None:
+            v = v + r
+            e = e + U32 * v.abs()
     return _store16(v, e, q)
 
 
@@ -208,6 +269,178 @@ def fc(x, w, b, q=True):
     en = e_y.norm(dim=1, keepdim=True)
     e = (e_y + out.abs() * en) / (nrm - en) + (w.shape[0] + 4) * U32 * out.abs()
     return out, e
+
+
+# ------------------------------------------------------------------------------------------------- Darknet ops
+def maxpool(x, size, stride, q=True):
+    """Darknet max-pool, NHWC, same-upper padding with -inf (out = ceil(in / stride), the smaller half of the padding
+    on top / left; oracle.nets._same_upper_pool).  Exact: a max of fp16 values is stored unchanged."""
+    x = _d(x)
+    h, w = x.shape[1:3]
+    ho, wo = -(-h // stride), -(-w // stride)
+    ph, pw = max((ho - 1) * stride + size - h, 0), max((wo - 1) * stride + size - w, 0)
+    xp = F.pad(_nchw(x), (pw // 2, pw - pw // 2, ph // 2, ph - ph // 2), value=float('-inf'))
+    want = _nhwc(F.max_pool2d(xp, size, stride))
+    return want, torch.zeros_like(want)
+
+
+def upsample(x, stride=2, q=True):
+    """Nearest upsample, NHWC: a copy (exact)."""
+    x = _d(x)
+    want = x.repeat_interleave(stride, 1).repeat_interleave(stride, 2)
+    return want, torch.zeros_like(want)
+
+
+def copy(x, q=True):
+    """A route source copied into its concat slice: exact."""
+    x = _d(x)
+    return x, torch.zeros_like(x)
+
+
+def add_act(a, b, act='linear', q=True):
+    """fm_add_act_strided (Darknet shortcut): act(a + b) with an fp32 add (one rounding, u32 |a + b|), the fp32
+    activation (_act_bound), fp16 store."""
+    v = _d(a) + _d(b)
+    v, e = _act_bound(v, U32 * v.abs(), act)
+    return _store16(v, e, q)
+
+
+def _f32(v):
+    """Round to fp32 (round to nearest even), back in float64.  For fp32 operands, the float64 result of + - * /
+    rounded once to fp32 is the correctly rounded fp32 result (53 >= 2 * 24 + 2), so a chain of _f32(a op b)
+    restates a chain of fp32 _rn operations exactly."""
+    return v.to(torch.float32).to(D)
+
+
+def _div(a, b):
+    """a / b correctly rounded: torch's CUDA division by a Python scalar multiplies by its reciprocal, which is not
+    (and can move a later fp32 rounding by an ulp), so the divisor is made a tensor."""
+    return a / torch.full_like(a, b)
+
+
+def decode64(head, anchors, scale_x_y, input_wh, num_classes, new_coords, size=(1.0, 1.0), offset=(0.0, 0.0)):
+    """csrc/detect.cu yolo_decode_filter_kernel in float64: head (A (5 + C), H, W) planar, the values the kernel read
+    (fp16 or fp32).  Returns (want, bound), each (A H W, 8) in candidate order (anchor, row, column):
+    columns px, py, pw, ph (pixels: scaled by `size`, minus `offset`), box_prob, class_id, cls_prob -- the dense
+    row the kernel writes -- and the score box_prob * cls_prob that meets conf_thresh.
+
+    new_coords: every step of the kernel is an fp32 _rn operation on exactly representable inputs, restated with
+    _f32 after each operation: exact, bound 0.
+    old coords: the sigmoids and exp go through __expf (relative error d = 2^-21 + |t| 2^-23).  The reference is the
+    exact real-number result; each later fp32 operation adds u32 of its result, and the input errors propagate
+    linearly (sigmoid with slope <= 1 in the relative sense, exp relative)."""
+    t = _d(head)
+    A = len(anchors) // 2
+    C = num_classes
+    _, H, W = t.shape
+    t = t.reshape(A, 5 + C, H, W)
+    cls = t[:, 5:]
+    best = cls.max(1).values
+    ids = torch.arange(C, device=t.device)[None, :, None, None]
+    class_id = torch.where(cls == best[:, None], ids, C).min(1).values      # the first maximum (the strict '>' scan)
+    col = torch.arange(W, dtype=D, device=t.device)[None, None, :]
+    row = torch.arange(H, dtype=D, device=t.device)[None, :, None]
+    aw = torch.tensor([float(a) for a in anchors[0::2]], dtype=D, device=t.device).to(torch.float32).to(D)
+    ah = torch.tensor([float(a) for a in anchors[1::2]], dtype=D, device=t.device).to(torch.float32).to(D)
+    aw, ah = aw[:, None, None], ah[:, None, None]
+    s = float(torch.tensor(scale_x_y, dtype=torch.float32))
+    iw, ih = float(input_wh[0]), float(input_wh[1])
+    sw, sh = (float(torch.tensor(v, dtype=torch.float32)) for v in size)
+    ox, oy = (float(torch.tensor(v, dtype=torch.float32)) for v in offset)
+    hs = float(_f32(torch.tensor(s - 1.0, dtype=D))) * 0.5              # __fmul_rn(s - 1.0f, 0.5f): exact halving
+    z = torch.zeros_like(best)
+    if new_coords:
+        f = _f32
+        cls_prob, box_prob = best, t[:, 4]
+        bw = f(_div(f(f(f(t[:, 2] * t[:, 2]) * 4.0) * aw), iw))
+        bh = f(_div(f(f(f(t[:, 3] * t[:, 3]) * 4.0) * ah), ih))
+        bx = f(_div(f(col + f(f(s * t[:, 0]) - hs)), W))
+        by = f(_div(f(row + f(f(s * t[:, 1]) - hs)), H))
+        bx, by = f(bx - f(bw * 0.5)), f(by - f(bh * 0.5))                 # halving is exact
+        px, py = f(f(bx * sw) - ox), f(f(by * sh) - oy)
+        pw, ph = f(bw * sw), f(bh * sh)
+        score = f(box_prob * cls_prob)
+        want = [px, py, pw, ph, box_prob, class_id.to(D), cls_prob, score]
+        bound = [z] * 8
+    else:
+        def sig(x):
+            g = torch.sigmoid(x)
+            return g, g * (_expf_rel(x) + 2 * U32)       # __expf(-x), 1 + n and the IEEE division
+
+        cls_prob, e_cls = sig(best)
+        box_prob, e_box = sig(t[:, 4])
+        ex, e_ex = sig(t[:, 0])
+        ey, e_ey = sig(t[:, 1])
+        bw = torch.exp(t[:, 2]) * aw / iw
+        bh = torch.exp(t[:, 3]) * ah / ih
+        e_bw = bw * (_expf_rel(t[:, 2]) + 3 * U32)        # __expf, the product by the anchor, the division
+        e_bh = bh * (_expf_rel(t[:, 3]) + 3 * U32)
+
+        def centre(cell, e, e_e, n):
+            a = s * e
+            ea = s * e_e + U32 * a.abs()
+            a = a - hs
+            ea = ea + U32 * a.abs()
+            a = cell + a
+            ea = ea + U32 * a.abs()
+            return a / n, ea / n + U32 * (a / n).abs()
+
+        bx, e_bx = centre(col, ex, e_ex, W)
+        by, e_by = centre(row, ey, e_ey, H)
+        bx, by = bx - bw / 2, by - bh / 2
+        e_bx, e_by = e_bx + e_bw / 2 + 2 * U32 * bx.abs(), e_by + e_bh / 2 + 2 * U32 * by.abs()
+
+        def pix(v, e, sc, off):
+            p = v * sc
+            ep = e * sc + U32 * p.abs()
+            return p - off, ep + U32 * (p - off).abs()
+
+        px, e_px = pix(bx, e_bx, sw, ox)
+        py, e_py = pix(by, e_by, sh, oy)
+        pw, e_pw = pix(bw, e_bw, sw, 0.0)
+        ph, e_ph = pix(bh, e_bh, sh, 0.0)
+        score = box_prob * cls_prob
+        e_score = e_box * cls_prob + e_cls * box_prob + e_box * e_cls + U32 * score
+        # the fp32 values stored: one more rounding of each (u32 relative)
+        want = [px, py, pw, ph, box_prob, class_id.to(D), cls_prob, score]
+        bound = [e_px, e_py, e_pw, e_ph, e_box, z, e_cls, e_score]
+        bound = [e + U32 * v.abs() if j != 5 else e for j, (v, e) in enumerate(zip(want, bound))]
+    want = torch.stack([v.expand(A, H, W) for v in want], -1).reshape(-1, 8)
+    bound = torch.stack([v.expand(A, H, W) for v in bound], -1).reshape(-1, 8)
+    return want, bound
+
+
+def run_darknet64(layers, weights, x, q=False):
+    """Composes the Darknet ops over a layer list of models/darknet.py (the semantics of oracle.nets.run_darknet).
+    x: (1, 3, H, W).  Returns the raw head tensors [(5 + C) A, H, W] float64."""
+    res, _ = darknet.infer_shapes(layers, x.shape[1], x.shape[2], x.shape[3])
+    outs, heads = [], []
+    cur = _nhwc(_d(x))
+    for i, l in enumerate(res):
+        t = l['type']
+        if t == 'convolutional':
+            w, b = weights[i]
+            k = l['size']
+            cur = conv(cur, w, b, l.get('stride', 1), k // 2 if l.get('pad', 0) else 0, l.get('activation', 'linear'),
+                       q=q)[0]
+        elif t == 'maxpool':
+            cur = maxpool(cur, l['size'], l['stride'])[0]
+        elif t == 'upsample':
+            cur = upsample(cur, l['stride'])[0]
+        elif t == 'shortcut':
+            cur = add_act(cur, outs[l['from_abs']], l.get('activation', 'linear'), q=q)[0]
+        elif t == 'route':
+            g, gid = l.get('groups', 1), l.get('group_id', 0)
+            parts = []
+            for s_ in l['layers_abs']:
+                o = outs[s_]
+                c = o.shape[-1] // g
+                parts.append(o[..., gid * c:(gid + 1) * c])
+            cur = torch.cat(parts, -1) if len(parts) > 1 else parts[0]
+        elif t == 'yolo':
+            heads.append(_nchw(cur)[0].clone())
+        outs.append(cur)
+    return heads
 
 
 # ------------------------------------------------------------------------------------------------- fused units
