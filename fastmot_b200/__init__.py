@@ -9,4 +9,5 @@ from .tracker import MultiTracker, DeviceEmbeddings
 from .detector import YOLODetector, PublicDetector, DET_DTYPE
 from .feature_extractor import FeatureExtractor
 from .mot import MOT
+from .multistream import MultiStreamMOT
 from . import models

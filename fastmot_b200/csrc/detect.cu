@@ -6,21 +6,28 @@
 //            rect.py:48-57 (to_tlbr), :21-32 (aspect_ratio, area).
 // The reference copies all K0 decoded candidates to the host and filters there; here only the D survivors
 // (48 B each) leave the device.
+//
+// Every kernel handles a batch of images: image b owns its own segment of each buffer (heads + b * head_stride,
+// dense rows + b * cand_stride, keys + b * key_cap, counter[b], mask + b * key_cap * words, outputs + b * max_out,
+// out_count[b], status[b]) and the grid carries b.  The one-image entries launch the same kernels with one image, so
+// a batched image's keys, rows and detections are those of the one-image path on the same head slice, and NMS never
+// compares boxes of different images.
 #include "common.cuh"
 #include "../../include/fastmot_b200.h"
 
-int fm_launch_nms_scan(const unsigned long long* keys, const float* dense, const int* counter, int key_cap,
-                       const unsigned long long* mask, int words, double max_area, double min_ar, int max_out,
-                       double* out_tlbr, long long* out_label, double* out_conf, int* out_count, int* status,
-                       cudaStream_t s);
+int fm_launch_nms_scan(int batch, const unsigned long long* keys, const float* dense, int cand_stride,
+                       const int* counter, int key_cap, const unsigned long long* mask, int words, double max_area,
+                       double min_ar, int max_out, double* out_tlbr, long long* out_label, double* out_conf,
+                       int* out_count, int* status, cudaStream_t s);
 
 namespace {
 
 __device__ __forceinline__ float sigmoidf_fast(float x) { return 1.0f / (1.0f + __expf(-x)); }
 
-// One thread per (anchor, cell).  Input NCHW-style head tensor [(5+C)*A, H, W] in fp32 or fp16.
+// One thread per (anchor, cell); blockIdx.y = image.  Input NCHW-style head tensor [(5+C)*A, H, W] in fp32 or fp16.
 template <typename T>
-__global__ void yolo_decode_filter_kernel(const T* __restrict__ in, int yolo_w, int yolo_h, int num_anchors,
+__global__ void yolo_decode_filter_kernel(const T* __restrict__ in, long long head_stride, int cand_stride,
+                                          int yolo_w, int yolo_h, int num_anchors,
                                           FmYoloHead head, int num_classes, int input_w, int input_h, int new_coords,
                                           int nhwc,
                                           int cand_base, const unsigned char* __restrict__ label_mask,
@@ -30,6 +37,11 @@ __global__ void yolo_decode_filter_kernel(const T* __restrict__ in, int yolo_w, 
     const int total = yolo_w * yolo_h;
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= total * num_anchors) return;
+    const int img = blockIdx.y;
+    in += img * head_stride;
+    dense += (size_t)img * cand_stride * 8;
+    keys += (size_t)img * key_cap;
+    counter += img;
     const int info_len = 5 + num_classes;
     const int anchor = idx / total, cell = idx - anchor * total;
     // planar [(5+C)*A, H, W] (the TensorRT plugin's input) or channels-last [H, W, (5+C)*A] (our conv engine)
@@ -91,11 +103,14 @@ __global__ void yolo_decode_filter_kernel(const T* __restrict__ in, int yolo_w, 
     }
 }
 
-// Single-CTA bitonic sort of up to 16384 keys in shared memory.
+// Bitonic sort of up to 16384 keys in shared memory, one CTA per image.
 __global__ void __launch_bounds__(1024) sort_keys_kernel(unsigned long long* __restrict__ keys,
                                                           const int* __restrict__ counter, int key_cap,
                                                           int* __restrict__ status) {
     extern __shared__ unsigned long long sk[];
+    keys += (size_t)blockIdx.x * key_cap;
+    counter += blockIdx.x;
+    status += blockIdx.x;
     int n = *counter;
     if (n > key_cap) {
         if (threadIdx.x == 0) status[0] = 1;   // overflow: host raises
@@ -139,13 +154,18 @@ __device__ __forceinline__ bool diou_suppresses(const float* a, const float* b, 
     return iou - pow(d / c, 0.6) > thresh;
 }
 
-// mask[i][w] bit b set  <=>  sorted candidate j = 64 w + b (j > i, same class) is suppressed by i.
+// mask[i][w] bit b set  <=>  sorted candidate j = 64 w + b (j > i, same class) is suppressed by i.  blockIdx.y = image.
 __global__ void __launch_bounds__(64) nms_mask_kernel(const unsigned long long* __restrict__ keys,
-                                                       const float* __restrict__ dense,
+                                                       const float* __restrict__ dense, int cand_stride,
                                                        const int* __restrict__ counter, int key_cap, double thresh,
                                                        unsigned long long* __restrict__ mask, int mask_words) {
     __shared__ float sb[64][4];
     __shared__ int scls[64];
+    const int img = blockIdx.y;
+    keys += (size_t)img * key_cap;
+    dense += (size_t)img * cand_stride * 8;
+    counter += img;
+    mask += (size_t)img * key_cap * mask_words;
     int n = min(*counter, key_cap);
     const int nb = (n + 63) >> 6;
     const int ntiles = nb * nb;
@@ -226,6 +246,28 @@ __global__ void __launch_bounds__(32) nms_scan_kernel(const unsigned long long* 
 
 }  // namespace
 
+static int launch_decode(const void* head_out, int batch, long long head_stride, int cand_stride, int is_fp16, int nhwc,
+                         int yolo_w, int yolo_h, int num_anchors, const FmYoloHead& head, int num_classes, int input_w,
+                         int input_h, int new_coords, int cand_base, const unsigned char* label_mask,
+                         double conf_thresh, float size_w, float size_h, float off_x, float off_y, float* dense,
+                         unsigned long long* keys, int* counter, int key_cap, void* stream, const char* what) {
+    int total = yolo_w * yolo_h * num_anchors;
+    if (total <= 0) return FM_OK;
+    dim3 grid(fm_cdiv(total, 128), batch);
+    if (is_fp16)
+        yolo_decode_filter_kernel<__half><<<grid, 128, 0, (cudaStream_t)stream>>>(
+            (const __half*)head_out, head_stride, cand_stride, yolo_w, yolo_h, num_anchors, head, num_classes, input_w,
+            input_h, new_coords, nhwc, cand_base, label_mask, conf_thresh, size_w, size_h, off_x, off_y, dense, keys,
+            counter, key_cap);
+    else
+        yolo_decode_filter_kernel<float><<<grid, 128, 0, (cudaStream_t)stream>>>(
+            (const float*)head_out, head_stride, cand_stride, yolo_w, yolo_h, num_anchors, head, num_classes, input_w,
+            input_h, new_coords, nhwc, cand_base, label_mask, conf_thresh, size_w, size_h, off_x, off_y, dense, keys,
+            counter, key_cap);
+    FM_CHECK_LAUNCH(what);
+    return FM_OK;
+}
+
 extern "C" int fm_yolo_decode_filter(const void* head_out, int is_fp16, int nhwc, int yolo_w, int yolo_h, int num_anchors,
                                      const FmYoloHead* head, int num_classes, int input_w, int input_h,
                                      int new_coords, int cand_base, const unsigned char* label_mask,
@@ -234,19 +276,27 @@ extern "C" int fm_yolo_decode_filter(const void* head_out, int is_fp16, int nhwc
     FM_REQUIRE(head != nullptr, "fm_yolo_decode_filter: head is NULL");
     FM_REQUIRE(num_anchors <= FM_MAX_ANCHORS, "fm_yolo_decode_filter: too many anchors");
     FM_REQUIRE(cand_base + yolo_w * yolo_h * num_anchors <= (1 << 24), "fm_yolo_decode_filter: > 2^24 candidates");
-    int total = yolo_w * yolo_h * num_anchors;
-    if (total <= 0) return FM_OK;
-    dim3 grid(fm_cdiv(total, 128));
-    if (is_fp16)
-        yolo_decode_filter_kernel<__half><<<grid, 128, 0, (cudaStream_t)stream>>>(
-            (const __half*)head_out, yolo_w, yolo_h, num_anchors, *head, num_classes, input_w, input_h, new_coords,
-            nhwc, cand_base, label_mask, conf_thresh, size_w, size_h, off_x, off_y, dense, keys, counter, key_cap);
-    else
-        yolo_decode_filter_kernel<float><<<grid, 128, 0, (cudaStream_t)stream>>>(
-            (const float*)head_out, yolo_w, yolo_h, num_anchors, *head, num_classes, input_w, input_h, new_coords,
-            nhwc, cand_base, label_mask, conf_thresh, size_w, size_h, off_x, off_y, dense, keys, counter, key_cap);
-    FM_CHECK_LAUNCH("fm_yolo_decode_filter");
-    return FM_OK;
+    return launch_decode(head_out, 1, 0, 0, is_fp16, nhwc, yolo_w, yolo_h, num_anchors, *head, num_classes, input_w,
+                         input_h, new_coords, cand_base, label_mask, conf_thresh, size_w, size_h, off_x, off_y, dense,
+                         keys, counter, key_cap, stream, "fm_yolo_decode_filter");
+}
+
+extern "C" int fm_yolo_decode_filter_batch(const void* head_out, int batch, long long head_stride, int is_fp16,
+                                           int nhwc, int yolo_w, int yolo_h, int num_anchors, const FmYoloHead* head,
+                                           int num_classes, int input_w, int input_h, int new_coords, int cand_base,
+                                           int cand_stride, const unsigned char* label_mask, double conf_thresh,
+                                           float size_w, float size_h, float off_x, float off_y, float* dense,
+                                           unsigned long long* keys, int* counters, int key_cap, void* stream) {
+    FM_REQUIRE(head != nullptr, "fm_yolo_decode_filter_batch: head is NULL");
+    FM_REQUIRE(num_anchors <= FM_MAX_ANCHORS, "fm_yolo_decode_filter_batch: too many anchors");
+    FM_REQUIRE(batch > 0 && batch <= 65535, "fm_yolo_decode_filter_batch: batch must be in [1, 65535]");
+    FM_REQUIRE(cand_base + yolo_w * yolo_h * num_anchors <= cand_stride && cand_stride <= (1 << 24),
+               "fm_yolo_decode_filter_batch: the head's candidates do not fit in cand_stride (<= 2^24) rows per image");
+    FM_REQUIRE(head_stride >= (long long)yolo_w * yolo_h * num_anchors * (5 + num_classes),
+               "fm_yolo_decode_filter_batch: head_stride is smaller than one image's head");
+    return launch_decode(head_out, batch, head_stride, cand_stride, is_fp16, nhwc, yolo_w, yolo_h, num_anchors, *head,
+                         num_classes, input_w, input_h, new_coords, cand_base, label_mask, conf_thresh, size_w, size_h,
+                         off_x, off_y, dense, keys, counters, key_cap, stream, "fm_yolo_decode_filter_batch");
 }
 
 extern "C" long long fm_nms_mask_bytes(int key_cap) {
@@ -254,11 +304,10 @@ extern "C" long long fm_nms_mask_bytes(int key_cap) {
     return (long long)key_cap * words * 8;
 }
 
-extern "C" int fm_diou_nms_filter(unsigned long long* keys, const float* dense, const int* counter, int key_cap,
-                                  double nms_thresh, double max_area, double min_aspect_ratio,
-                                  unsigned long long* mask, int max_out, double* out_tlbr, long long* out_label,
-                                  double* out_conf, int* out_count, int* status, void* stream) {
-    FM_REQUIRE(key_cap > 0 && key_cap <= 16384, "fm_diou_nms_filter: key_cap must be in (0, 16384]");
+static int launch_nms(int batch, unsigned long long* keys, const float* dense, int cand_stride, const int* counter,
+                      int key_cap, double nms_thresh, double max_area, double min_aspect_ratio,
+                      unsigned long long* mask, int max_out, double* out_tlbr, long long* out_label, double* out_conf,
+                      int* out_count, int* status, void* stream) {
     static bool attr_set = false;
     if (!attr_set) {
         cudaFuncSetAttribute(sort_keys_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 16384 * 8);
@@ -267,14 +316,36 @@ extern "C" int fm_diou_nms_filter(unsigned long long* keys, const float* dense, 
     cudaStream_t s = (cudaStream_t)stream;
     int np2 = 1;
     while (np2 < key_cap) np2 <<= 1;
-    cudaMemsetAsync(status, 0, sizeof(int), s);
-    sort_keys_kernel<<<1, 1024, (size_t)np2 * 8, s>>>(keys, counter, key_cap, status);
+    cudaMemsetAsync(status, 0, sizeof(int) * batch, s);
+    sort_keys_kernel<<<batch, 1024, (size_t)np2 * 8, s>>>(keys, counter, key_cap, status);
     FM_CHECK_LAUNCH("sort_keys_kernel");
     const int words = (key_cap + 63) / 64;
-    nms_mask_kernel<<<FM_NUM_SMS * 8, 64, 0, s>>>(keys, dense, counter, key_cap, nms_thresh, mask, words);
+    nms_mask_kernel<<<dim3(FM_NUM_SMS * 8, batch), 64, 0, s>>>(keys, dense, cand_stride, counter, key_cap, nms_thresh,
+                                                                mask, words);
     FM_CHECK_LAUNCH("nms_mask_kernel");
-    fm_launch_nms_scan(keys, dense, counter, key_cap, mask, words, max_area, min_aspect_ratio, max_out, out_tlbr,
-                       out_label, out_conf, out_count, status, s);   // blocked scan, detect_nms.cu
+    fm_launch_nms_scan(batch, keys, dense, cand_stride, counter, key_cap, mask, words, max_area, min_aspect_ratio,
+                       max_out, out_tlbr, out_label, out_conf, out_count, status, s);   // blocked scan, detect_nms.cu
     FM_CHECK_LAUNCH("nms_scan_kernel");
     return FM_OK;
+}
+
+extern "C" int fm_diou_nms_filter(unsigned long long* keys, const float* dense, const int* counter, int key_cap,
+                                  double nms_thresh, double max_area, double min_aspect_ratio,
+                                  unsigned long long* mask, int max_out, double* out_tlbr, long long* out_label,
+                                  double* out_conf, int* out_count, int* status, void* stream) {
+    FM_REQUIRE(key_cap > 0 && key_cap <= 16384, "fm_diou_nms_filter: key_cap must be in (0, 16384]");
+    return launch_nms(1, keys, dense, 0, counter, key_cap, nms_thresh, max_area, min_aspect_ratio, mask, max_out,
+                      out_tlbr, out_label, out_conf, out_count, status, stream);
+}
+
+extern "C" int fm_diou_nms_filter_batch(int batch, unsigned long long* keys, const float* dense, int cand_stride,
+                                        const int* counters, int key_cap, double nms_thresh, double max_area,
+                                        double min_aspect_ratio, unsigned long long* mask, int max_out,
+                                        double* out_tlbr, long long* out_label, double* out_conf, int* out_count,
+                                        int* status, void* stream) {
+    FM_REQUIRE(key_cap > 0 && key_cap <= 16384, "fm_diou_nms_filter_batch: key_cap must be in (0, 16384]");
+    FM_REQUIRE(batch > 0 && batch <= 65535, "fm_diou_nms_filter_batch: batch must be in [1, 65535]");
+    FM_REQUIRE(cand_stride > 0 && cand_stride <= (1 << 24), "fm_diou_nms_filter_batch: cand_stride must be in (0, 2^24]");
+    return launch_nms(batch, keys, dense, cand_stride, counters, key_cap, nms_thresh, max_area, min_aspect_ratio, mask,
+                      max_out, out_tlbr, out_label, out_conf, out_count, status, stream);
 }

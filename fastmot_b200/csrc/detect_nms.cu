@@ -33,8 +33,9 @@ __device__ __forceinline__ NmsOut nms_final_filter(const unsigned long long* __r
     return o;
 }
 
+// one CTA per image (blockIdx.x): the image's segments of keys, dense rows, mask and outputs (detect.cu)
 __global__ void __launch_bounds__(NMS_THREADS) nms_scan_blocked_kernel(const unsigned long long* __restrict__ keys,
-                                                                        const float* __restrict__ dense,
+                                                                        const float* __restrict__ dense, int cand_stride,
                                                                         const int* __restrict__ counter, int key_cap,
                                                                         const unsigned long long* __restrict__ mask,
                                                                         int mask_words, double max_area, double min_ar,
@@ -45,6 +46,16 @@ __global__ void __launch_bounds__(NMS_THREADS) nms_scan_blocked_kernel(const uns
     extern __shared__ unsigned long long sm[];   // removed[nw] | keep[nw] | okbits (u32 x 2nw) | prefix (i32 x 2nw)
     __shared__ unsigned long long s_kept;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int img = blockIdx.x;
+    keys += (size_t)img * key_cap;
+    dense += (size_t)img * cand_stride * 8;
+    counter += img;
+    mask += (size_t)img * key_cap * mask_words;
+    out_tlbr += (size_t)img * max_out * 4;
+    out_label += (size_t)img * max_out;
+    out_conf += (size_t)img * max_out;
+    out_count += img;
+    status += img;
     const int n = min(*counter, key_cap);
     const int nw = (n + 63) >> 6;
     unsigned long long* removed = sm;
@@ -137,11 +148,12 @@ __global__ void __launch_bounds__(NMS_THREADS) nms_scan_blocked_kernel(const uns
 
 }  // namespace
 
-int fm_launch_nms_scan(const unsigned long long* keys, const float* dense, const int* counter, int key_cap,
-                       const unsigned long long* mask, int words, double max_area, double min_ar, int max_out,
-                       double* out_tlbr, long long* out_label, double* out_conf, int* out_count, int* status,
-                       cudaStream_t s) {
-    nms_scan_blocked_kernel<<<1, NMS_THREADS, (size_t)(4 * words + 4) * 8, s>>>(keys, dense, counter, key_cap, mask, words,
+int fm_launch_nms_scan(int batch, const unsigned long long* keys, const float* dense, int cand_stride,
+                       const int* counter, int key_cap, const unsigned long long* mask, int words, double max_area,
+                       double min_ar, int max_out, double* out_tlbr, long long* out_label, double* out_conf,
+                       int* out_count, int* status, cudaStream_t s) {
+    nms_scan_blocked_kernel<<<batch, NMS_THREADS, (size_t)(4 * words + 4) * 8, s>>>(keys, dense, cand_stride, counter,
+                                                                     key_cap, mask, words,
                                                                      max_area, min_ar, max_out, out_tlbr, out_label,
                                                                      out_conf, out_count, status);
     return 0;

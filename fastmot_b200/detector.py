@@ -70,7 +70,10 @@ class YOLODetector(Detector):
                  min_aspect_ratio=1.2,
                  max_dets=4096,
                  key_cap=16384,
-                 engine=None):
+                 engine=None,
+                 batch=1):
+        """batch = B > 1: the detector runs B frames of this size per forward (detect_batch_async /
+        postprocess_batch); key_cap and max_dets then hold per image."""
         super().__init__(size)
         self._lib = _lib.require_device()
         self.model = models.YOLO.get_model(model)
@@ -94,6 +97,8 @@ class YOLODetector(Detector):
         self.roi, self.upscaled_sz, self.bbox_offset = letterbox_geometry(size, self.input_wh, self.model.LETTERBOX)
 
         dev = torch.device("cuda")
+        assert batch >= 1
+        B = self.batch = batch
         self.max_dets, self.key_cap = max_dets, key_cap
         self.heads = []
         k0 = 0
@@ -107,26 +112,36 @@ class YOLODetector(Detector):
             k0 += na * (in_w // factor) * (in_h // factor)
         self.num_candidates = k0
         self._label_mask_dev = torch.as_tensor(self.label_mask.astype(np.uint8)).to(dev)
-        self._dense = torch.zeros(k0, 8, dtype=torch.float32, device=dev)
-        self._keys = torch.zeros(key_cap, dtype=torch.int64, device=dev)
-        self._counter = torch.zeros(1, dtype=torch.int32, device=dev)
-        self._mask = torch.zeros(int(self._lib.fm_nms_mask_bytes(key_cap)), dtype=torch.uint8, device=dev)
+        # image b owns rows [b k0, (b + 1) k0) of the candidate table, keys [b key_cap, (b + 1) key_cap), one mask
+        # segment and output rows [b max_dets, (b + 1) max_dets)
+        self._dense = torch.zeros(B * k0, 8, dtype=torch.float32, device=dev)
+        self._keys = torch.zeros(B * key_cap, dtype=torch.int64, device=dev)
+        self._counter = torch.zeros(B, dtype=torch.int32, device=dev)
+        self._mask = torch.zeros(B * int(self._lib.fm_nms_mask_bytes(key_cap)), dtype=torch.uint8, device=dev)
         # outputs packed in one block -> one D2H
-        self._out_tlbr = torch.zeros(max_dets, 4, dtype=torch.float64, device=dev)
-        self._out_label = torch.zeros(max_dets, dtype=torch.int64, device=dev)
-        self._out_conf = torch.zeros(max_dets, dtype=torch.float64, device=dev)
-        self._out_meta = torch.zeros(4, dtype=torch.int32, device=dev)   # [count, status, n_candidates, -]
-        self._h_tlbr = torch.zeros(max_dets, 4, dtype=torch.float64).pin_memory()
-        self._h_label = torch.zeros(max_dets, dtype=torch.int64).pin_memory()
-        self._h_conf = torch.zeros(max_dets, dtype=torch.float64).pin_memory()
-        self._h_meta = torch.zeros(4, dtype=torch.int32).pin_memory()
-        self.inp = torch.zeros(in_h, in_w, 8, dtype=torch.float16, device=dev)   # NHWC8
+        self._out_tlbr = torch.zeros(B * max_dets, 4, dtype=torch.float64, device=dev)
+        self._out_label = torch.zeros(B * max_dets, dtype=torch.int64, device=dev)
+        self._out_conf = torch.zeros(B * max_dets, dtype=torch.float64, device=dev)
+        # [count, status, n_candidates, -] (batch: [count[B], status[B], n_candidates[B]])
+        self._out_meta = torch.zeros(max(4, 3 * B), dtype=torch.int32, device=dev)
+        self._h_tlbr = torch.zeros(B * max_dets, 4, dtype=torch.float64).pin_memory()
+        self._h_label = torch.zeros(B * max_dets, dtype=torch.int64).pin_memory()
+        self._h_conf = torch.zeros(B * max_dets, dtype=torch.float64).pin_memory()
+        self._h_meta = torch.zeros(max(4, 3 * B), dtype=torch.int32).pin_memory()
+        lead = () if B == 1 else (B,)
+        self.inp = torch.zeros(lead + (in_h, in_w, 8), dtype=torch.float16, device=dev)   # NHWC8
         self._uploader = FrameUploader(size)
+        self._uploaders = [self._uploader] + [None] * (B - 1)    # built on the first host frame of their slot
+        self._frame_tab_h = torch.zeros(B, dtype=torch.int64).pin_memory()     # frame pointers of detect_batch_async
+        self._frame_tab = torch.zeros(B, dtype=torch.int64, device=dev)
+        self._frame_tab_ev = None
         self.frame_dev = None
         self._done = torch.cuda.Event()
         if engine is None:
             from .engine import build_yolo_engine
-            engine = build_yolo_engine(self.model)
+            engine = build_yolo_engine(self.model, batch=B)
+        if getattr(engine, 'batch', 1) != B:
+            raise ValueError(f"the engine runs {getattr(engine, 'batch', 1)} images per forward, the detector {B}")
         self.backend = engine
 
     # ------------------------------------------------------------------
@@ -192,6 +207,97 @@ class YOLODetector(Detector):
         dets['label'] = self._h_label.numpy()[:n]
         dets['conf'] = self._h_conf.numpy()[:n]
         return dets.view(np.recarray)
+
+    # ------------------------------------------------------------------ batch > 1
+    def preprocess_batch(self, frames_dev):
+        """Letterbox of the B frames (HxWx3 u8 cuda tensors of this detector's size) into self.inp, one launch."""
+        B = self.batch
+        if len(frames_dev) != B:
+            raise ValueError(f"expected {B} frames, got {len(frames_dev)}")
+        want = (self.size[1], self.size[0], 3)
+        for f in frames_dev:
+            if tuple(f.shape) != want or f.dtype != torch.uint8 or not f.is_contiguous() or not f.is_cuda:
+                raise ValueError(f"every frame must be a contiguous uint8 cuda tensor of shape {want}")
+        if self._frame_tab_ev is not None:
+            self._frame_tab_ev.synchronize()        # the previous table upload has left the pinned block
+        self._frame_tab_h.copy_(torch.tensor([f.data_ptr() for f in frames_dev], dtype=torch.int64))
+        self._frame_tab.copy_(self._frame_tab_h, non_blocking=True)
+        self._frame_tab_ev = torch.cuda.Event()
+        self._frame_tab_ev.record()
+        rx, ry, rw, rh = self.roi
+        rc = self._lib.fm_letterbox_preproc_batch(ptr(self._frame_tab), B, self.size[0], self.size[1],
+                                                  self.input_wh[0], self.input_wh[1], rx, ry, rw, rh, ptr(self.inp),
+                                                  stream_ptr())
+        _lib.check(rc, "fm_letterbox_preproc_batch")
+
+    def detect_batch_async(self, frames):
+        """detect_async for B frames at once: one letterbox launch, one conv-stack forward over the B images, one
+        decode launch per head and one batched NMS; `postprocess_batch` waits for the results."""
+        if len(frames) != self.batch:
+            raise ValueError(f"expected {self.batch} frames, got {len(frames)}")
+        self.frames_dev = [f if torch.is_tensor(f) else self._upload(b, f) for b, f in enumerate(frames)]
+        self.preprocess_batch(self.frames_dev)
+        heads = self.backend.forward(self.inp)
+        self.postprocess_heads_batch_async(heads)
+
+    def _upload(self, b, frame):
+        if self._uploaders[b] is None:
+            self._uploaders[b] = FrameUploader(self.size)
+        return self._uploaders[b].upload(frame)
+
+    def postprocess_heads_batch_async(self, head_tensors):
+        """Decode + filter + NMS of B images' fp16 NHWC heads [B][H][W][(5+C)*A] ([H][W][(5+C)*A] at B = 1)."""
+        s = stream_ptr()
+        B, k0 = self.batch, self.num_candidates
+        self._counter.zero_()
+        lib = self._lib
+        for hd, t in zip(self.heads, head_tensors):
+            assert t.is_contiguous() and t.dtype == torch.float16 and t.numel() % B == 0
+            rc = lib.fm_yolo_decode_filter_batch(ptr(t), B, t.numel() // B, 1, 1, hd['w'], hd['h'], hd['na'],
+                                                 C.byref(hd['head']), self.model.NUM_CLASSES, self.input_wh[0],
+                                                 self.input_wh[1], 1 if self.model.NEW_COORDS else 0, hd['base'], k0,
+                                                 ptr(self._label_mask_dev), float(self.conf_thresh),
+                                                 float(self.upscaled_sz[0]), float(self.upscaled_sz[1]),
+                                                 float(self.bbox_offset[0]), float(self.bbox_offset[1]),
+                                                 ptr(self._dense), ptr(self._keys), ptr(self._counter), self.key_cap, s)
+            _lib.check(rc, "fm_yolo_decode_filter_batch")
+        meta = self._out_meta
+        rc = lib.fm_diou_nms_filter_batch(B, ptr(self._keys), ptr(self._dense), k0, ptr(self._counter), self.key_cap,
+                                          float(self.nms_thresh), float(self.max_area), float(self.min_aspect_ratio),
+                                          ptr(self._mask), self.max_dets, ptr(self._out_tlbr), ptr(self._out_label),
+                                          ptr(self._out_conf), ptr(meta[:B]), ptr(meta[B:2 * B]), s)
+        _lib.check(rc, "fm_diou_nms_filter_batch")
+        lib.fm_memcpy_async(ptr(meta[2 * B:3 * B]), ptr(self._counter), 4 * B, s)
+        self._h_meta.copy_(meta, non_blocking=True)
+        self._h_tlbr.copy_(self._out_tlbr, non_blocking=True)
+        self._h_label.copy_(self._out_label, non_blocking=True)
+        self._h_conf.copy_(self._out_conf, non_blocking=True)
+        self._done.record()
+
+    def postprocess_batch(self):
+        """Waits for detect_batch_async; returns a list of B np.recarray[DET_DTYPE], one per frame, each ordered as
+        `postprocess` orders one frame's detections."""
+        self._done.synchronize()
+        B, md = self.batch, self.max_dets
+        meta = self._h_meta.numpy()
+        count, status, n_cand = meta[:B], meta[B:2 * B], meta[2 * B:3 * B]
+        for b in range(B):
+            if status[b] == 2:
+                raise RuntimeError(f"image {b}: more than max_dets = {md} boxes survived NMS and the area / aspect "
+                                   "filters; raise max_dets (no silent truncation)")
+            if status[b] != 0:
+                raise RuntimeError(f"image {b}: {n_cand[b]} candidates passed conf_thresh but key_cap is "
+                                   f"{self.key_cap}; raise key_cap (no silent truncation)")
+        self.last_num_candidates = [int(v) for v in n_cand]
+        out = []
+        for b in range(B):
+            n, r0 = int(count[b]), b * md
+            dets = np.zeros(n, DET_DTYPE)
+            dets['tlbr'] = self._h_tlbr.numpy()[r0:r0 + n]
+            dets['label'] = self._h_label.numpy()[r0:r0 + n]
+            dets['conf'] = self._h_conf.numpy()[r0:r0 + n]
+            out.append(dets.view(np.recarray))
+        return out
 
 
 

@@ -162,15 +162,21 @@ class _Net:
 
 
 class YoloEngine(_Net):
-    """Darknet graph executor.  forward(inp NHWC8 fp16) -> list of head tensors [H, W, (5+C)*A] fp16."""
+    """Darknet graph executor.  forward(inp NHWC8 fp16) -> list of head tensors [H, W, (5+C)*A] fp16.
+
+    With batch = B > 1 every tensor gains a leading image dimension: the input is [B][H][W][8], the heads are
+    [B][H][W][(5+C)*A], and every launch covers the B images (conv descriptors, pools, upsample and route copies get
+    n = B; route buffers are [B][h][w][c]).  Each conv keeps the path the kernels' own `supported` checks pick at n = B."""
     heads_nhwc = True
 
-    def __init__(self, layers, input_hw, weights, use_tc=True, use_graph=False):
+    def __init__(self, layers, input_hw, weights, use_tc=True, use_graph=False, batch=1):
         super().__init__(use_tc, use_graph)
         H, W = input_hw
+        B = self.batch = batch
+        lead = () if B == 1 else (B,)        # batch 1 keeps the unbatched shapes
         self.layers, self.shapes = darknet.infer_shapes(layers, 3, H, W)
-        self.inp = torch.zeros(H, W, IN_C_PAD, dtype=torch.float16, device=self.dev)
-        self.flops = darknet.count_flops(layers, 3, H, W)
+        self.inp = torch.zeros(lead + (H, W, IN_C_PAD), dtype=torch.float16, device=self.dev)
+        self.flops = darknet.count_flops(layers, 3, H, W) * B
         L = self.layers
         n = len(L)
         # ---- plan: which layers are written straight into a concat buffer ----
@@ -188,7 +194,7 @@ class YoloEngine(_Net):
         def route_buf(i):
             if i not in bufs:
                 c, h, w = self.shapes[i]
-                bufs[i] = torch.zeros(h, w, c, dtype=torch.float16, device=self.dev)
+                bufs[i] = torch.zeros(lead + (h, w, c), dtype=torch.float16, device=self.dev)
             return bufs[i]
 
         self.views = []     # per layer: (tensor, c, c_stride, c_off, h, w)
@@ -228,7 +234,7 @@ class YoloEngine(_Net):
                 ri, off = home[i]
                 out = (route_buf(ri), c, self.shapes[ri][0], off, h, w)
             elif t in ('convolutional', 'maxpool', 'upsample', 'shortcut') and i not in self.fused_shortcuts:
-                out = (torch.zeros(h, w, c, dtype=torch.float16, device=self.dev), c, c, 0, h, w)
+                out = (torch.zeros(lead + (h, w, c), dtype=torch.float16, device=self.dev), c, c, 0, h, w)
             else:
                 out = None
             src = self.views[i - 1] if i else (self.inp, IN_C_PAD, IN_C_PAD, 0, H, W)
@@ -242,7 +248,7 @@ class YoloEngine(_Net):
                 bd = torch.as_tensor(bs).to(self.dev).float().contiguous()
                 self.params[i] = (wd, bd)
                 pad = k // 2 if l.get('pad', 0) else 0
-                d = _conv_desc(1, src[4], src[5], cin, src[2], src[3], h, w, c, out[2], out[3], k, l.get('stride', 1),
+                d = _conv_desc(B, src[4], src[5], cin, src[2], src[3], h, w, c, out[2], out[3], k, l.get('stride', 1),
                                pad, _ACT[l.get('activation', 'linear')])
                 if i + 1 in self.fused_shortcuts:
                     fr = L[i + 1]['from_abs']
@@ -264,14 +270,14 @@ class YoloEngine(_Net):
                     if prev is not None and ksz > prev[0]:
                         ksz, psrc, pj = ksz - prev[0] + 1, prev[1], prev[2]
                     spp_prev[key] = (l['size'], out, i)
-                self._add('fm_maxpool', ptr(psrc[0]), ptr(out[0]), 1, psrc[4], psrc[5], psrc[1], psrc[2], psrc[3],
+                self._add('fm_maxpool', ptr(psrc[0]), ptr(out[0]), B, psrc[4], psrc[5], psrc[1], psrc[2], psrc[3],
                           ksz, l['stride'], out[2], out[3])
                 # ins[0] is the declared source; a composed SPP pool also reads the smaller pool's output
                 self.trace.append(TraceEntry('maxpool', (i,), [vw(i - 1)] + ([vw(pj)] if pj != i - 1 else []),
                                              [vw(i, out)], {'size': l['size'], 'src': i - 1, 'stride': l['stride'],
                                                             'launch_size': ksz, 'launch_src': pj}))
             elif t == 'upsample':
-                self._add('fm_upsample_copy', ptr(src[0]), ptr(out[0]), 1, src[4], src[5], src[1], src[2], src[3],
+                self._add('fm_upsample_copy', ptr(src[0]), ptr(out[0]), B, src[4], src[5], src[1], src[2], src[3],
                           l['stride'], out[2], out[3])
                 self.trace.append(TraceEntry('upsample', (i,), [vw(i - 1)], [vw(i, out)], {'stride': l['stride']}))
             elif t == 'shortcut' and i in self.fused_shortcuts:
@@ -279,7 +285,7 @@ class YoloEngine(_Net):
             elif t == 'shortcut':
                 a, b = self.views[i - 1], self.views[l['from_abs']]
                 self._add('fm_add_act_strided', ptr(a[0]), a[2], a[3], ptr(b[0]), b[2], b[3], ptr(out[0]), out[2],
-                          out[3], h * w, c, _ACT[l.get('activation', 'linear')])
+                          out[3], B * h * w, c, _ACT[l.get('activation', 'linear')])
                 self.trace.append(TraceEntry('shortcut', (i,), [vw(i - 1), vw(l['from_abs'])], [vw(i, out)]))
             elif t == 'route':
                 srcs = l['layers_abs']
@@ -295,7 +301,7 @@ class YoloEngine(_Net):
                         sv = self.views[s]
                         cs = sv[1] // g
                         if home.get(s, (None,))[0] != i:
-                            self._add('fm_upsample_copy', ptr(sv[0]), ptr(buf), 1, sv[4], sv[5], cs, sv[2],
+                            self._add('fm_upsample_copy', ptr(sv[0]), ptr(buf), B, sv[4], sv[5], cs, sv[2],
                                       sv[3] + l.get('group_id', 0) * cs, 1, c, off)
                             self.trace.append(TraceEntry(
                                 'copy', (i,), [vw(s, (sv[0], cs, sv[2], sv[3] + l.get('group_id', 0) * cs) + sv[4:])],
@@ -315,9 +321,9 @@ class YoloEngine(_Net):
         return self.heads
 
 
-def build_yolo_engine(model, weights=None, use_tc=True, use_graph=True, head_obj_bias=-5.0):
-    """Engine for a `models.YOLO` descriptor.  Without a Darknet .weights file the weights are synthetic
-    (seeded He-normal, detection-prior objectness bias) — there are no trained weights offline."""
+def build_yolo_engine(model, weights=None, use_tc=True, use_graph=True, head_obj_bias=-5.0, batch=1):
+    """Engine for a `models.YOLO` descriptor (`batch` images per forward).  Without a Darknet .weights file the
+    weights are synthetic (seeded He-normal, detection-prior objectness bias) — there are no trained weights offline."""
     if isinstance(model.CFG, str) and model.CFG in darknet.BUILDERS:
         layers = darknet.BUILDERS[model.CFG](num_classes=model.NUM_CLASSES,
                                              anchors_per_head=len(model.ANCHORS[0]) // 2)
@@ -334,7 +340,7 @@ def build_yolo_engine(model, weights=None, use_tc=True, use_graph=True, head_obj
             weights = darknet.synthetic_weights(layers, 3, head_obj_bias=head_obj_bias,
                                                 num_classes=model.NUM_CLASSES,
                                                 head_gain=float(os.environ.get("FM_SYNTH_HEAD_GAIN", 1.0)))
-    return YoloEngine(layers, model.INPUT_SHAPE[1:], weights, use_tc=use_tc, use_graph=use_graph)
+    return YoloEngine(layers, model.INPUT_SHAPE[1:], weights, use_tc=use_tc, use_graph=use_graph, batch=batch)
 
 
 class OSNetEngine(_Net):

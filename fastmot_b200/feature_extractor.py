@@ -33,6 +33,10 @@ class FeatureExtractor:
         self._uploader = None
         self.last_num_features = 0
         self._out = None
+        self._splits = None         # per-stream crop offsets of the last extract_multi_async
+        self._frame_idx_host = torch.zeros(max_crops, dtype=torch.int32).pin_memory()
+        self._frame_idx_dev = torch.zeros(max_crops, dtype=torch.int32, device=dev)
+        self._frame_tab_host = self._frame_tab_dev = None
 
     def _engine(self, n):
         """Engines are planned per batch bucket (multiples of 8 crops): a frame pays for its own crops, not for
@@ -58,6 +62,7 @@ class FeatureExtractor:
         n = len(tlbrs)
         self.last_num_features = n
         self._out = None
+        self._splits = None
         if n == 0:
             return
         if n > self.max_crops:
@@ -79,8 +84,52 @@ class FeatureExtractor:
         _lib.check(rc, "fm_roi_resize_norm")
         self._out = eng.forward(n)
 
+    def extract_multi_async(self, frames, tlbrs_per_stream):
+        """extract_async over several streams at once: frames[s] (HxWx3 u8 cuda tensors, all of one size) with its
+        boxes tlbrs_per_stream[s].  All crops are cut in one launch and run through one OSNet forward (the batch
+        buckets of extract_async hold the sum over streams); `postprocess` then returns one slice per stream."""
+        if len(frames) != len(tlbrs_per_stream):
+            raise ValueError("one box array per frame")
+        tl = [np.ascontiguousarray(t, np.float64).reshape(-1, 4) for t in tlbrs_per_stream]
+        counts = [len(t) for t in tl]
+        n = sum(counts)
+        self.last_num_features = n
+        self._out = None
+        self._splits = np.concatenate([[0], np.cumsum(counts)]).astype(int)
+        if n == 0:
+            return
+        if n > self.max_crops:
+            raise MemoryError(f"{n} crops > max_crops {self.max_crops}")
+        h, w = frames[0].shape[:2]
+        for f in frames:
+            if not torch.is_tensor(f) or not f.is_cuda or f.dtype != torch.uint8 or tuple(f.shape) != (h, w, 3) \
+                    or not f.is_contiguous():
+                raise ValueError(f"every frame must be a contiguous uint8 cuda tensor of shape {(h, w, 3)}")
+        if self._frame_tab_host is None or self._frame_tab_host.numel() < len(frames):
+            self._frame_tab_host = torch.zeros(len(frames), dtype=torch.int64).pin_memory()
+            self._frame_tab_dev = torch.zeros(len(frames), dtype=torch.int64, device=self._frame_idx_dev.device)
+        eng = self._engine(n)
+        self._tlbr_host[:n] = torch.as_tensor(np.concatenate(tl))
+        self._tlbr_dev[:n].copy_(self._tlbr_host[:n], non_blocking=True)
+        self._frame_idx_host[:n] = torch.as_tensor(np.repeat(np.arange(len(frames), dtype=np.int32), counts))
+        self._frame_idx_dev[:n].copy_(self._frame_idx_host[:n], non_blocking=True)
+        self._frame_tab_host[:len(frames)] = torch.tensor([f.data_ptr() for f in frames], dtype=torch.int64)
+        self._frame_tab_dev[:len(frames)].copy_(self._frame_tab_host[:len(frames)], non_blocking=True)
+        c, ih, iw = self.model.INPUT_SHAPE
+        rc = self._lib.fm_roi_resize_norm_multi(ptr(self._frame_tab_dev), ptr(self._frame_idx_dev), w, h,
+                                                ptr(self._tlbr_dev), n, iw, ih, eng.inp_layout, ptr(eng.inp),
+                                                stream_ptr())
+        _lib.check(rc, "fm_roi_resize_norm_multi")
+        self._out = eng.forward(n)
+
     def postprocess(self):
-        """Returns DeviceEmbeddings (N, feature_dim) — numpy-convertible, rows L2-normalised."""
+        """Returns DeviceEmbeddings (N, feature_dim) — numpy-convertible, rows L2-normalised.  After
+        extract_multi_async: a list with one entry per stream, each a view of that stream's rows of the shared
+        output (no copy)."""
+        if self._splits is not None:
+            sp = self._splits
+            return [DeviceEmbeddings(self._out[a:b]) if b > a else np.empty((0, self.feature_dim))
+                    for a, b in zip(sp[:-1], sp[1:])]
         if self.last_num_features == 0:
             return np.empty((0, self.feature_dim))
         return DeviceEmbeddings(self._out)

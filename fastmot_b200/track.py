@@ -37,10 +37,9 @@ class AverageFeature:
 
 
 class Track:
-    _count = 0
-
-    def __init__(self, frame_id, tlbr, pool, label, confirm_hits=1, buffer_size=30, slot=None):
-        self.trk_id = self.next_id()
+    def __init__(self, trk_id, frame_id, tlbr, pool, label, confirm_hits=1, buffer_size=30, slot=None):
+        # the id comes from the owning MultiTracker: every tracker numbers its own tracks from 1
+        self.trk_id = trk_id
         self._pool = pool
         self.slot = pool.acquire() if slot is None else slot
         self.start_frame = frame_id
@@ -125,8 +124,3 @@ class Track:
 
     def mark_missed(self):
         self.age += 1
-
-    @staticmethod
-    def next_id():
-        Track._count += 1
-        return Track._count

@@ -100,6 +100,7 @@ class MultiTracker:
         self._lib = _lib.require_device()
         self.tracks = {}
         self.hist_tracks = OrderedDict()
+        self._last_id = 0           # track ids are per tracker: several trackers in one process never share them
         self.kf = KalmanFilter(**vars(kalman_filter_cfg))
         self.pool = TrackPool(pool_capacity, feat_dim)
         from .flow import Flow
@@ -144,7 +145,7 @@ class MultiTracker:
         for trk in self.hist_tracks.values():
             self.pool.release(trk.slot)
         self.hist_tracks.clear()
-        Track._count = 0
+        self._last_id = 0
 
     def _clear_tracks(self):
         for trk in self.tracks.values():
@@ -158,7 +159,8 @@ class MultiTracker:
             return
         new = []
         for det_id in det_ids:
-            trk = Track(frame_id, det_tlbr_host[det_id].copy(), self.pool, int(det_labels_host[det_id]),
+            self._last_id += 1
+            trk = Track(self._last_id, frame_id, det_tlbr_host[det_id].copy(), self.pool, int(det_labels_host[det_id]),
                         self.confirm_hits)
             self.tracks[trk.trk_id] = trk
             new.append(trk)
