@@ -9,5 +9,6 @@ from .tracker import MultiTracker, DeviceEmbeddings
 from .detector import YOLODetector, PublicDetector, DET_DTYPE
 from .feature_extractor import FeatureExtractor
 from .mot import MOT
+from .multicamera import MultiCameraMOT
 from .multistream import MultiStreamMOT
 from . import models

@@ -78,6 +78,11 @@ class FmYoloHead(C.Structure):
     _fields_ = [("anchors", c_f * 12), ("scale_x_y", c_f)]
 
 
+class FmFrameGeom(C.Structure):
+    _fields_ = [("frame", c_p), ("w", c_i), ("h", c_i), ("roi_x", c_i), ("roi_y", c_i), ("roi_w", c_i),
+                ("roi_h", c_i), ("size_w", c_f), ("size_h", c_f), ("off_x", c_f), ("off_y", c_f)]
+
+
 # name -> (restype, argtypes); kept in one table so tests can check it against the header
 SIGNATURES = {
     "fm_last_error": (C.c_char_p, []),
@@ -104,6 +109,10 @@ SIGNATURES = {
     "fm_roi_resize_norm": (c_i, [c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p]),
     "fm_letterbox_preproc_batch": (c_i, [c_p, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_p, c_p]),
     "fm_roi_resize_norm_multi": (c_i, [c_p, c_p, c_i, c_i, c_p, c_i, c_i, c_i, c_i, c_p, c_p]),
+    "fm_letterbox_preproc_geom": (c_i, [c_p, c_i, c_i, c_i, c_p, c_p]),
+    "fm_roi_resize_norm_geom": (c_i, [c_p, c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p]),
+    "fm_yolo_decode_filter_geom": (c_i, [c_p, c_i, c_ll, c_i, c_i, c_i, c_i, c_i, C.POINTER(FmYoloHead), c_i, c_i,
+                                          c_i, c_i, c_i, c_i, c_p, c_d, c_p, c_p, c_p, c_p, c_i, c_p]),
     "fm_yolo_decode_filter_batch": (c_i, [c_p, c_i, c_ll, c_i, c_i, c_i, c_i, c_i, C.POINTER(FmYoloHead), c_i, c_i,
                                            c_i, c_i, c_i, c_i, c_p, c_d, c_f, c_f, c_f, c_f, c_p, c_p, c_p, c_i, c_p]),
     "fm_diou_nms_filter_batch": (c_i, [c_i, c_p, c_p, c_i, c_p, c_i, c_d, c_d, c_d, c_p, c_i, c_p, c_p, c_p, c_p, c_p,

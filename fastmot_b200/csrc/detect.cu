@@ -11,7 +11,8 @@
 // dense rows + b * cand_stride, keys + b * key_cap, counter[b], mask + b * key_cap * words, outputs + b * max_out,
 // out_count[b], status[b]) and the grid carries b.  The one-image entries launch the same kernels with one image, so
 // a batched image's keys, rows and detections are those of the one-image path on the same head slice, and NMS never
-// compares boxes of different images.
+// compares boxes of different images.  The *_geom entry reads each image's pixel scale and letterbox offset from a
+// device FmFrameGeom table instead of taking one for the whole batch (images of different frame sizes).
 #include "common.cuh"
 #include "../../include/fastmot_b200.h"
 
@@ -32,7 +33,7 @@ __global__ void yolo_decode_filter_kernel(const T* __restrict__ in, long long he
                                           int nhwc,
                                           int cand_base, const unsigned char* __restrict__ label_mask,
                                           double conf_thresh, float size_w, float size_h, float off_x, float off_y,
-                                          float* __restrict__ dense, unsigned long long* __restrict__ keys,
+                                          const FmFrameGeom* __restrict__ geom, float* __restrict__ dense, unsigned long long* __restrict__ keys,
                                           int* __restrict__ counter, int key_cap) {
     const int total = yolo_w * yolo_h;
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -87,6 +88,10 @@ __global__ void yolo_decode_filter_kernel(const T* __restrict__ in, long long he
     // floats is exact, so its f32 rounding is __fmul_rn; likewise the f32 rounding of the f64 difference is __fsub_rn.
     // Written as f64 casts the compiler lowered both to plain mul.f32 / sub.f32, which ptxas contracted into one FFMA:
     // the product was never rounded and py differed from the reference by up to half an ulp of by * size_h.
+    if (geom != nullptr) {
+        const FmFrameGeom& g = geom[img];
+        size_w = g.size_w; size_h = g.size_h; off_x = g.off_x; off_y = g.off_y;
+    }
     const float px = __fsub_rn(__fmul_rn(bx, size_w), off_x);
     const float py = __fsub_rn(__fmul_rn(by, size_h), off_y);
     const float pw = __fmul_rn(bw, size_w);
@@ -249,21 +254,22 @@ __global__ void __launch_bounds__(32) nms_scan_kernel(const unsigned long long* 
 static int launch_decode(const void* head_out, int batch, long long head_stride, int cand_stride, int is_fp16, int nhwc,
                          int yolo_w, int yolo_h, int num_anchors, const FmYoloHead& head, int num_classes, int input_w,
                          int input_h, int new_coords, int cand_base, const unsigned char* label_mask,
-                         double conf_thresh, float size_w, float size_h, float off_x, float off_y, float* dense,
-                         unsigned long long* keys, int* counter, int key_cap, void* stream, const char* what) {
+                         double conf_thresh, float size_w, float size_h, float off_x, float off_y,
+                         const FmFrameGeom* geom, float* dense, unsigned long long* keys, int* counter, int key_cap,
+                         void* stream, const char* what) {
     int total = yolo_w * yolo_h * num_anchors;
     if (total <= 0) return FM_OK;
     dim3 grid(fm_cdiv(total, 128), batch);
     if (is_fp16)
         yolo_decode_filter_kernel<__half><<<grid, 128, 0, (cudaStream_t)stream>>>(
             (const __half*)head_out, head_stride, cand_stride, yolo_w, yolo_h, num_anchors, head, num_classes, input_w,
-            input_h, new_coords, nhwc, cand_base, label_mask, conf_thresh, size_w, size_h, off_x, off_y, dense, keys,
-            counter, key_cap);
+            input_h, new_coords, nhwc, cand_base, label_mask, conf_thresh, size_w, size_h, off_x, off_y, geom, dense,
+            keys, counter, key_cap);
     else
         yolo_decode_filter_kernel<float><<<grid, 128, 0, (cudaStream_t)stream>>>(
             (const float*)head_out, head_stride, cand_stride, yolo_w, yolo_h, num_anchors, head, num_classes, input_w,
-            input_h, new_coords, nhwc, cand_base, label_mask, conf_thresh, size_w, size_h, off_x, off_y, dense, keys,
-            counter, key_cap);
+            input_h, new_coords, nhwc, cand_base, label_mask, conf_thresh, size_w, size_h, off_x, off_y, geom, dense,
+            keys, counter, key_cap);
     FM_CHECK_LAUNCH(what);
     return FM_OK;
 }
@@ -277,8 +283,8 @@ extern "C" int fm_yolo_decode_filter(const void* head_out, int is_fp16, int nhwc
     FM_REQUIRE(num_anchors <= FM_MAX_ANCHORS, "fm_yolo_decode_filter: too many anchors");
     FM_REQUIRE(cand_base + yolo_w * yolo_h * num_anchors <= (1 << 24), "fm_yolo_decode_filter: > 2^24 candidates");
     return launch_decode(head_out, 1, 0, 0, is_fp16, nhwc, yolo_w, yolo_h, num_anchors, *head, num_classes, input_w,
-                         input_h, new_coords, cand_base, label_mask, conf_thresh, size_w, size_h, off_x, off_y, dense,
-                         keys, counter, key_cap, stream, "fm_yolo_decode_filter");
+                         input_h, new_coords, cand_base, label_mask, conf_thresh, size_w, size_h, off_x, off_y, nullptr,
+                         dense, keys, counter, key_cap, stream, "fm_yolo_decode_filter");
 }
 
 extern "C" int fm_yolo_decode_filter_batch(const void* head_out, int batch, long long head_stride, int is_fp16,
@@ -296,7 +302,26 @@ extern "C" int fm_yolo_decode_filter_batch(const void* head_out, int batch, long
                "fm_yolo_decode_filter_batch: head_stride is smaller than one image's head");
     return launch_decode(head_out, batch, head_stride, cand_stride, is_fp16, nhwc, yolo_w, yolo_h, num_anchors, *head,
                          num_classes, input_w, input_h, new_coords, cand_base, label_mask, conf_thresh, size_w, size_h,
-                         off_x, off_y, dense, keys, counters, key_cap, stream, "fm_yolo_decode_filter_batch");
+                         off_x, off_y, nullptr, dense, keys, counters, key_cap, stream, "fm_yolo_decode_filter_batch");
+}
+
+extern "C" int fm_yolo_decode_filter_geom(const void* head_out, int batch, long long head_stride, int is_fp16,
+                                          int nhwc, int yolo_w, int yolo_h, int num_anchors, const FmYoloHead* head,
+                                          int num_classes, int input_w, int input_h, int new_coords, int cand_base,
+                                          int cand_stride, const unsigned char* label_mask, double conf_thresh,
+                                          const FmFrameGeom* geom, float* dense, unsigned long long* keys,
+                                          int* counters, int key_cap, void* stream) {
+    FM_REQUIRE(head != nullptr, "fm_yolo_decode_filter_geom: head is NULL");
+    FM_REQUIRE(geom != nullptr, "fm_yolo_decode_filter_geom: geometry table is NULL");
+    FM_REQUIRE(num_anchors <= FM_MAX_ANCHORS, "fm_yolo_decode_filter_geom: too many anchors");
+    FM_REQUIRE(batch > 0 && batch <= 65535, "fm_yolo_decode_filter_geom: batch must be in [1, 65535]");
+    FM_REQUIRE(cand_base + yolo_w * yolo_h * num_anchors <= cand_stride && cand_stride <= (1 << 24),
+               "fm_yolo_decode_filter_geom: the head's candidates do not fit in cand_stride (<= 2^24) rows per image");
+    FM_REQUIRE(head_stride >= (long long)yolo_w * yolo_h * num_anchors * (5 + num_classes),
+               "fm_yolo_decode_filter_geom: head_stride is smaller than one image's head");
+    return launch_decode(head_out, batch, head_stride, cand_stride, is_fp16, nhwc, yolo_w, yolo_h, num_anchors, *head,
+                         num_classes, input_w, input_h, new_coords, cand_base, label_mask, conf_thresh, 0.f, 0.f, 0.f,
+                         0.f, geom, dense, keys, counters, key_cap, stream, "fm_yolo_decode_filter_geom");
 }
 
 extern "C" long long fm_nms_mask_bytes(int key_cap) {

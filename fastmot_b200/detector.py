@@ -72,8 +72,10 @@ class YOLODetector(Detector):
                  key_cap=16384,
                  engine=None,
                  batch=1):
-        """batch = B > 1: the detector runs B frames of this size per forward (detect_batch_async /
-        postprocess_batch); key_cap and max_dets then hold per image."""
+        """batch = B > 1: the detector runs up to B frames per forward (detect_batch_async / postprocess_batch);
+        key_cap and max_dets then hold per image.  B frames of `size` run the batch-B engine with this size's
+        geometry; any other set of 1..B frames (any sizes) runs the engine of its own batch k, which shares the batch-B
+        engine's weights and buffers, with each frame's geometry taken from its shape."""
         super().__init__(size)
         self._lib = _lib.require_device()
         self.model = models.YOLO.get_model(model)
@@ -135,6 +137,13 @@ class YOLODetector(Detector):
         self._frame_tab_h = torch.zeros(B, dtype=torch.int64).pin_memory()     # frame pointers of detect_batch_async
         self._frame_tab = torch.zeros(B, dtype=torch.int64, device=dev)
         self._frame_tab_ev = None
+        # per-frame geometry (one FmFrameGeom row per image) of the frames that are not B frames of `size`
+        self._geom_bytes = C.sizeof(_lib.FmFrameGeom)
+        self._geom_h = torch.zeros(B * self._geom_bytes, dtype=torch.uint8).pin_memory()
+        self._geom = torch.zeros(B * self._geom_bytes, dtype=torch.uint8, device=dev)
+        self._geom_ev = None
+        self._geometry = {tuple(size): (self.roi, self.upscaled_sz, self.bbox_offset)}
+        self._k = B                 # images of the last detect_batch_async
         self.frame_dev = None
         self._done = torch.cuda.Event()
         if engine is None:
@@ -143,6 +152,7 @@ class YOLODetector(Detector):
         if getattr(engine, 'batch', 1) != B:
             raise ValueError(f"the engine runs {getattr(engine, 'batch', 1)} images per forward, the detector {B}")
         self.backend = engine
+        self._engines = {B: engine}     # batch k -> engine; k < B share the batch-B engine's resources
 
     # ------------------------------------------------------------------
     def preprocess(self, frame_dev):
@@ -231,66 +241,140 @@ class YOLODetector(Detector):
         _lib.check(rc, "fm_letterbox_preproc_batch")
 
     def detect_batch_async(self, frames):
-        """detect_async for B frames at once: one letterbox launch, one conv-stack forward over the B images, one
-        decode launch per head and one batched NMS; `postprocess_batch` waits for the results."""
-        if len(frames) != self.batch:
-            raise ValueError(f"expected {self.batch} frames, got {len(frames)}")
+        """detect_async for 1..B frames at once: one letterbox launch, one conv-stack forward over the k images, one
+        decode launch per head and one batched NMS; `postprocess_batch` waits for the results.  B frames of this
+        detector's size take the batch-B engine; any other k frames (HxWx3 u8 of any sizes) the batch-k engine, each
+        frame with the letterbox and box geometry of its own size."""
+        k = len(frames)
+        if not 1 <= k <= self.batch:
+            raise ValueError(f"expected 1 to {self.batch} frames, got {k}")
         self.frames_dev = [f if torch.is_tensor(f) else self._upload(b, f) for b, f in enumerate(frames)]
-        self.preprocess_batch(self.frames_dev)
-        heads = self.backend.forward(self.inp)
-        self.postprocess_heads_batch_async(heads)
+        want = (self.size[1], self.size[0], 3)
+        if k == self.batch and all(tuple(f.shape) == want for f in self.frames_dev):
+            self.preprocess_batch(self.frames_dev)
+            heads = self.backend.forward(self.inp)
+            self.postprocess_heads_batch_async(heads)
+            return
+        geom = self.preprocess_frames(self.frames_dev)
+        heads = self.engine(k).forward(self.inp[:k] if k > 1 else self.inp[0])
+        self.postprocess_heads_batch_async(heads, k, geom)
+
+    def engine(self, k):
+        """The conv stack at batch k (1 <= k <= B); k < B is built on first use and shares the batch-B engine's
+        weights, workspace and buffers (YoloEngine.with_batch)."""
+        if k not in self._engines:
+            if not 1 <= k < self.batch:
+                raise ValueError(f"batch {k} is outside 1..{self.batch}")
+            self._engines[k] = self.backend.with_batch(k)
+        return self._engines[k]
+
+    def build_engines(self):
+        """Builds the engines of every batch 1..B now rather than on first use."""
+        for k in range(1, self.batch + 1):
+            self.engine(k)
 
     def _upload(self, b, frame):
-        if self._uploaders[b] is None:
-            self._uploaders[b] = FrameUploader(self.size)
+        h, w = frame.shape[:2]
+        if self._uploaders[b] is None or self._uploaders[b].shape != (h, w, 3):
+            self._uploaders[b] = FrameUploader((w, h))
         return self._uploaders[b].upload(frame)
 
-    def postprocess_heads_batch_async(self, head_tensors):
-        """Decode + filter + NMS of B images' fp16 NHWC heads [B][H][W][(5+C)*A] ([H][W][(5+C)*A] at B = 1)."""
+    def geometry(self, wh):
+        """(roi, upscaled_sz, bbox_offset) of frames of size wh = (width, height) in this detector's input."""
+        wh = tuple(int(v) for v in wh)
+        if wh not in self._geometry:
+            self._geometry[wh] = letterbox_geometry(wh, self.input_wh, self.model.LETTERBOX)
+        return self._geometry[wh]
+
+    def preprocess_frames(self, frames_dev):
+        """Letterbox of k frames of any sizes (HxWx3 u8 cuda tensors) into self.inp[:k], one launch.  Uploads
+        their FmFrameGeom table (one copy from a pinned block) and returns it: the head decode reads it too."""
+        k = len(frames_dev)
+        if not 1 <= k <= self.batch:
+            raise ValueError(f"expected 1 to {self.batch} frames, got {k}")
+        rows = (_lib.FmFrameGeom * k)()
+        for r, f in zip(rows, frames_dev):
+            if f.dim() != 3 or f.shape[2] != 3 or f.dtype != torch.uint8 or not f.is_contiguous() or not f.is_cuda:
+                raise ValueError("every frame must be a contiguous HxWx3 uint8 cuda tensor")
+            h, w = f.shape[:2]
+            (rx, ry, rw, rh), up, off = self.geometry((w, h))
+            r.frame, r.w, r.h = f.data_ptr(), w, h
+            r.roi_x, r.roi_y, r.roi_w, r.roi_h = rx, ry, rw, rh
+            r.size_w, r.size_h, r.off_x, r.off_y = float(up[0]), float(up[1]), float(off[0]), float(off[1])
+        if self._geom_ev is not None:
+            self._geom_ev.synchronize()          # the previous table upload has left the pinned block
+        nb = k * self._geom_bytes
+        C.memmove(self._geom_h.data_ptr(), C.addressof(rows), nb)
+        self._geom[:nb].copy_(self._geom_h[:nb], non_blocking=True)
+        self._geom_ev = torch.cuda.Event()
+        self._geom_ev.record()
+        rc = self._lib.fm_letterbox_preproc_geom(ptr(self._geom), k, self.input_wh[0], self.input_wh[1],
+                                                 ptr(self.inp), stream_ptr())
+        _lib.check(rc, "fm_letterbox_preproc_geom")
+        return self._geom
+
+    def postprocess_heads_batch_async(self, head_tensors, k=None, geom=None):
+        """Decode + filter + NMS of k (default B) images' fp16 NHWC heads [k][H][W][(5+C)*A] ([H][W][(5+C)*A] at
+        k = 1).  geom: the device FmFrameGeom table of preprocess_frames (each image's own box geometry); without it
+        every image has this detector's size."""
         s = stream_ptr()
         B, k0 = self.batch, self.num_candidates
+        k = B if k is None else k
+        self._k = k
         self._counter.zero_()
         lib = self._lib
         for hd, t in zip(self.heads, head_tensors):
-            assert t.is_contiguous() and t.dtype == torch.float16 and t.numel() % B == 0
-            rc = lib.fm_yolo_decode_filter_batch(ptr(t), B, t.numel() // B, 1, 1, hd['w'], hd['h'], hd['na'],
-                                                 C.byref(hd['head']), self.model.NUM_CLASSES, self.input_wh[0],
-                                                 self.input_wh[1], 1 if self.model.NEW_COORDS else 0, hd['base'], k0,
-                                                 ptr(self._label_mask_dev), float(self.conf_thresh),
-                                                 float(self.upscaled_sz[0]), float(self.upscaled_sz[1]),
-                                                 float(self.bbox_offset[0]), float(self.bbox_offset[1]),
-                                                 ptr(self._dense), ptr(self._keys), ptr(self._counter), self.key_cap, s)
-            _lib.check(rc, "fm_yolo_decode_filter_batch")
+            assert t.is_contiguous() and t.dtype == torch.float16 and t.numel() % k == 0
+            if geom is None:
+                rc = lib.fm_yolo_decode_filter_batch(ptr(t), k, t.numel() // k, 1, 1, hd['w'], hd['h'], hd['na'],
+                                                     C.byref(hd['head']), self.model.NUM_CLASSES, self.input_wh[0],
+                                                     self.input_wh[1], 1 if self.model.NEW_COORDS else 0, hd['base'],
+                                                     k0, ptr(self._label_mask_dev), float(self.conf_thresh),
+                                                     float(self.upscaled_sz[0]), float(self.upscaled_sz[1]),
+                                                     float(self.bbox_offset[0]), float(self.bbox_offset[1]),
+                                                     ptr(self._dense), ptr(self._keys), ptr(self._counter),
+                                                     self.key_cap, s)
+                _lib.check(rc, "fm_yolo_decode_filter_batch")
+            else:
+                rc = lib.fm_yolo_decode_filter_geom(ptr(t), k, t.numel() // k, 1, 1, hd['w'], hd['h'], hd['na'],
+                                                    C.byref(hd['head']), self.model.NUM_CLASSES, self.input_wh[0],
+                                                    self.input_wh[1], 1 if self.model.NEW_COORDS else 0, hd['base'],
+                                                    k0, ptr(self._label_mask_dev), float(self.conf_thresh), ptr(geom),
+                                                    ptr(self._dense), ptr(self._keys), ptr(self._counter),
+                                                    self.key_cap, s)
+                _lib.check(rc, "fm_yolo_decode_filter_geom")
         meta = self._out_meta
-        rc = lib.fm_diou_nms_filter_batch(B, ptr(self._keys), ptr(self._dense), k0, ptr(self._counter), self.key_cap,
+        rc = lib.fm_diou_nms_filter_batch(k, ptr(self._keys), ptr(self._dense), k0, ptr(self._counter), self.key_cap,
                                           float(self.nms_thresh), float(self.max_area), float(self.min_aspect_ratio),
                                           ptr(self._mask), self.max_dets, ptr(self._out_tlbr), ptr(self._out_label),
-                                          ptr(self._out_conf), ptr(meta[:B]), ptr(meta[B:2 * B]), s)
+                                          ptr(self._out_conf), ptr(meta[:k]), ptr(meta[B:B + k]), s)
         _lib.check(rc, "fm_diou_nms_filter_batch")
-        lib.fm_memcpy_async(ptr(meta[2 * B:3 * B]), ptr(self._counter), 4 * B, s)
+        lib.fm_memcpy_async(ptr(meta[2 * B:2 * B + k]), ptr(self._counter), 4 * k, s)
         self._h_meta.copy_(meta, non_blocking=True)
         self._h_tlbr.copy_(self._out_tlbr, non_blocking=True)
         self._h_label.copy_(self._out_label, non_blocking=True)
         self._h_conf.copy_(self._out_conf, non_blocking=True)
         self._done.record()
 
-    def postprocess_batch(self):
-        """Waits for detect_batch_async; returns a list of B np.recarray[DET_DTYPE], one per frame, each ordered as
-        `postprocess` orders one frame's detections."""
+    def postprocess_batch(self, names=None):
+        """Waits for detect_batch_async; returns a list of k np.recarray[DET_DTYPE], one per frame, each ordered as
+        `postprocess` orders one frame's detections.  An overflow raises and names image b as names[b] (default
+        'image b')."""
         self._done.synchronize()
-        B, md = self.batch, self.max_dets
+        B, k, md = self.batch, self._k, self.max_dets
         meta = self._h_meta.numpy()
-        count, status, n_cand = meta[:B], meta[B:2 * B], meta[2 * B:3 * B]
-        for b in range(B):
+        count, status, n_cand = meta[:k], meta[B:B + k], meta[2 * B:2 * B + k]
+        for b in range(k):
+            name = f"image {b}" if names is None else names[b]
             if status[b] == 2:
-                raise RuntimeError(f"image {b}: more than max_dets = {md} boxes survived NMS and the area / aspect "
+                raise RuntimeError(f"{name}: more than max_dets = {md} boxes survived NMS and the area / aspect "
                                    "filters; raise max_dets (no silent truncation)")
             if status[b] != 0:
-                raise RuntimeError(f"image {b}: {n_cand[b]} candidates passed conf_thresh but key_cap is "
+                raise RuntimeError(f"{name}: {n_cand[b]} candidates passed conf_thresh but key_cap is "
                                    f"{self.key_cap}; raise key_cap (no silent truncation)")
         self.last_num_candidates = [int(v) for v in n_cand]
         out = []
-        for b in range(B):
+        for b in range(k):
             n, r0 = int(count[b]), b * md
             dets = np.zeros(n, DET_DTYPE)
             dets['tlbr'] = self._h_tlbr.numpy()[r0:r0 + n]

@@ -90,7 +90,7 @@ class _Net:
     """Shared plumbing: recorded launches, optional CUDA-graph replay, conv dispatch (wgmma when supported)."""
     WS_BYTES = 32 << 20
 
-    def __init__(self, use_tc=True, use_graph=False):
+    def __init__(self, use_tc=True, use_graph=False, ws=None):
         self._lib = _lib.require_device()
         self.use_tc = use_tc
         self.use_graph = use_graph
@@ -102,7 +102,8 @@ class _Net:
         self.layer_bytes = 0        # algorithmic HBM bytes of the conv / depthwise layers (each tensor moved once)
         self.dev = torch.device("cuda")
         # split-K scratch of the wgmma conv: one per engine, so engines on different streams never share partials
-        self.ws = torch.empty(self.WS_BYTES, dtype=torch.uint8, device=self.dev)
+        # (`ws` given: an engine that only ever runs on the same stream as its owner, one after the other)
+        self.ws = ws if ws is not None else torch.empty(self.WS_BYTES, dtype=torch.uint8, device=self.dev)
 
     def _conv(self, desc, x, w, b, out, residual=None):
         """Records the conv on the path that supports it; returns that path: 'tma', 'tc' or 'simt'."""
@@ -166,16 +167,37 @@ class YoloEngine(_Net):
 
     With batch = B > 1 every tensor gains a leading image dimension: the input is [B][H][W][8], the heads are
     [B][H][W][(5+C)*A], and every launch covers the B images (conv descriptors, pools, upsample and route copies get
-    n = B; route buffers are [B][h][w][c]).  Each conv keeps the path the kernels' own `supported` checks pick at n = B."""
+    n = B; route buffers are [B][h][w][c]).  Each conv keeps the path the kernels' own `supported` checks pick at n = B.
+
+    share = an engine of the same network at a larger batch (see `with_batch`): this engine allocates nothing on the
+    device.  It runs on share's weights and split-K workspace, and its input, route and activation buffers are the
+    first B images of share's.  The plan below is deterministic, so both engines allocate the same buffers in the same
+    order and the i-th buffer of this engine is a prefix of share's i-th."""
     heads_nhwc = True
 
-    def __init__(self, layers, input_hw, weights, use_tc=True, use_graph=False, batch=1):
-        super().__init__(use_tc, use_graph)
+    def __init__(self, layers, input_hw, weights, use_tc=True, use_graph=False, batch=1, share=None):
+        if share is not None and not (1 <= batch < share.batch):
+            raise ValueError(f"a shared engine runs fewer images than its owner ({share.batch}), got batch {batch}")
+        super().__init__(use_tc, use_graph, ws=None if share is None else share.ws)
         H, W = input_hw
         B = self.batch = batch
+        self._src = (layers, tuple(input_hw))
         lead = () if B == 1 else (B,)        # batch 1 keeps the unbatched shapes
+        self._bufs = []                      # the device buffers in allocation order (share's, when shared)
+
+        def alloc(shape):
+            if share is None:
+                t = torch.zeros(lead + shape, dtype=torch.float16, device=self.dev)
+                self._bufs.append(t)
+                return t
+            if len(self._bufs) >= len(share._bufs) or tuple(share._bufs[len(self._bufs)].shape[1:]) != shape:
+                raise ValueError("the shared engine's buffer plan differs from its owner's")
+            t = share._bufs[len(self._bufs)]
+            self._bufs.append(t)
+            return t[:B] if B > 1 else t[0]
+
         self.layers, self.shapes = darknet.infer_shapes(layers, 3, H, W)
-        self.inp = torch.zeros(lead + (H, W, IN_C_PAD), dtype=torch.float16, device=self.dev)
+        self.inp = alloc((H, W, IN_C_PAD))
         self.flops = darknet.count_flops(layers, 3, H, W) * B
         L = self.layers
         n = len(L)
@@ -194,7 +216,7 @@ class YoloEngine(_Net):
         def route_buf(i):
             if i not in bufs:
                 c, h, w = self.shapes[i]
-                bufs[i] = torch.zeros(lead + (h, w, c), dtype=torch.float16, device=self.dev)
+                bufs[i] = alloc((h, w, c))
             return bufs[i]
 
         self.views = []     # per layer: (tensor, c, c_stride, c_off, h, w)
@@ -234,18 +256,21 @@ class YoloEngine(_Net):
                 ri, off = home[i]
                 out = (route_buf(ri), c, self.shapes[ri][0], off, h, w)
             elif t in ('convolutional', 'maxpool', 'upsample', 'shortcut') and i not in self.fused_shortcuts:
-                out = (torch.zeros(lead + (h, w, c), dtype=torch.float16, device=self.dev), c, c, 0, h, w)
+                out = (alloc((h, w, c)), c, c, 0, h, w)
             else:
                 out = None
             src = self.views[i - 1] if i else (self.inp, IN_C_PAD, IN_C_PAD, 0, H, W)
             if t == 'convolutional':
-                wt, bs = weights[i]
                 k = l['size']
                 cin = src[1]
-                if i == 0:   # physical input has IN_C_PAD channels (the extra ones are zero)
-                    wt = np.concatenate([wt, np.zeros(wt.shape[:3] + (IN_C_PAD - wt.shape[3],), np.float32)], -1)
-                wd = torch.as_tensor(np.ascontiguousarray(wt)).to(self.dev).half().contiguous()
-                bd = torch.as_tensor(bs).to(self.dev).float().contiguous()
+                if share is not None:
+                    wd, bd = share.params[i]
+                else:
+                    wt, bs = weights[i]
+                    if i == 0:   # physical input has IN_C_PAD channels (the extra ones are zero)
+                        wt = np.concatenate([wt, np.zeros(wt.shape[:3] + (IN_C_PAD - wt.shape[3],), np.float32)], -1)
+                    wd = torch.as_tensor(np.ascontiguousarray(wt)).to(self.dev).half().contiguous()
+                    bd = torch.as_tensor(bs).to(self.dev).float().contiguous()
                 self.params[i] = (wd, bd)
                 pad = k // 2 if l.get('pad', 0) else 0
                 d = _conv_desc(B, src[4], src[5], cin, src[2], src[3], h, w, c, out[2], out[3], k, l.get('stride', 1),
@@ -313,6 +338,17 @@ class YoloEngine(_Net):
                 assert out[2] == out[1] and out[3] == 0
                 self.heads.append(out[0])
             self.views.append(out)
+        if share is not None and len(self._bufs) != len(share._bufs):
+            raise ValueError("the shared engine's buffer plan differs from its owner's")
+
+    def with_batch(self, k, use_graph=None):
+        """The engine of this network at batch k < self.batch that shares this engine's device weights, split-K
+        workspace and buffers (the first k images of each): one more launch list (and graph), no activation memory.
+        Each conv keeps the path its kernel picks at n = k.  It overwrites this engine's buffers, so the two must run
+        one after the other on one stream."""
+        layers, input_hw = self._src
+        return YoloEngine(layers, input_hw, None, use_tc=self.use_tc,
+                          use_graph=self.use_graph if use_graph is None else use_graph, batch=k, share=self)
 
     def forward(self, inp):
         if inp.data_ptr() != self.inp.data_ptr():

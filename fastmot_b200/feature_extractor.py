@@ -7,6 +7,8 @@ crops + cv2.resize's on CPU threads and uploads 16 crops at a time) and run thro
 the embeddings stay on the GPU (`DeviceEmbeddings`) and feed the association kernels directly.  The reference's
 aliasing defect for > batch_size crops (SURVEY.md Appendix A) is not reproduced.
 """
+import ctypes as C
+
 import numpy as np
 import torch
 
@@ -36,7 +38,8 @@ class FeatureExtractor:
         self._splits = None         # per-stream crop offsets of the last extract_multi_async
         self._frame_idx_host = torch.zeros(max_crops, dtype=torch.int32).pin_memory()
         self._frame_idx_dev = torch.zeros(max_crops, dtype=torch.int32, device=dev)
-        self._frame_tab_host = self._frame_tab_dev = None
+        self._geom_host = self._geom_dev = None     # FmFrameGeom rows of extract_multi_async's frames
+        self._geom_ev = None
 
     def _engine(self, n):
         """Engines are planned per batch bucket (multiples of 8 crops): a frame pays for its own crops, not for
@@ -85,9 +88,10 @@ class FeatureExtractor:
         self._out = eng.forward(n)
 
     def extract_multi_async(self, frames, tlbrs_per_stream):
-        """extract_async over several streams at once: frames[s] (HxWx3 u8 cuda tensors, all of one size) with its
-        boxes tlbrs_per_stream[s].  All crops are cut in one launch and run through one OSNet forward (the batch
-        buckets of extract_async hold the sum over streams); `postprocess` then returns one slice per stream."""
+        """extract_async over several streams at once: frames[s] (HxWx3 u8 cuda tensors, each of its own size) with
+        its boxes tlbrs_per_stream[s].  All crops are cut in one launch, each clamped to its own frame, and run through
+        one OSNet forward (the batch buckets of extract_async hold the sum over streams); `postprocess` then returns
+        one slice per stream."""
         if len(frames) != len(tlbrs_per_stream):
             raise ValueError("one box array per frame")
         tl = [np.ascontiguousarray(t, np.float64).reshape(-1, 4) for t in tlbrs_per_stream]
@@ -100,26 +104,34 @@ class FeatureExtractor:
             return
         if n > self.max_crops:
             raise MemoryError(f"{n} crops > max_crops {self.max_crops}")
-        h, w = frames[0].shape[:2]
-        for f in frames:
-            if not torch.is_tensor(f) or not f.is_cuda or f.dtype != torch.uint8 or tuple(f.shape) != (h, w, 3) \
+        rows = (_lib.FmFrameGeom * len(frames))()
+        for r, f in zip(rows, frames):
+            if not torch.is_tensor(f) or not f.is_cuda or f.dtype != torch.uint8 or f.dim() != 3 or f.shape[2] != 3 \
                     or not f.is_contiguous():
-                raise ValueError(f"every frame must be a contiguous uint8 cuda tensor of shape {(h, w, 3)}")
-        if self._frame_tab_host is None or self._frame_tab_host.numel() < len(frames):
-            self._frame_tab_host = torch.zeros(len(frames), dtype=torch.int64).pin_memory()
-            self._frame_tab_dev = torch.zeros(len(frames), dtype=torch.int64, device=self._frame_idx_dev.device)
+                raise ValueError("every frame must be a contiguous HxWx3 uint8 cuda tensor")
+            r.frame, r.h, r.w = f.data_ptr(), f.shape[0], f.shape[1]
+        nb = C.sizeof(rows)
+        if self._geom_host is None or self._geom_host.numel() < nb:
+            if self._geom_ev is not None:
+                self._geom_ev.synchronize()
+            self._geom_host = torch.zeros(nb, dtype=torch.uint8).pin_memory()
+            self._geom_dev = torch.zeros(nb, dtype=torch.uint8, device=self._frame_idx_dev.device)
+            self._geom_ev = None
         eng = self._engine(n)
         self._tlbr_host[:n] = torch.as_tensor(np.concatenate(tl))
         self._tlbr_dev[:n].copy_(self._tlbr_host[:n], non_blocking=True)
         self._frame_idx_host[:n] = torch.as_tensor(np.repeat(np.arange(len(frames), dtype=np.int32), counts))
         self._frame_idx_dev[:n].copy_(self._frame_idx_host[:n], non_blocking=True)
-        self._frame_tab_host[:len(frames)] = torch.tensor([f.data_ptr() for f in frames], dtype=torch.int64)
-        self._frame_tab_dev[:len(frames)].copy_(self._frame_tab_host[:len(frames)], non_blocking=True)
+        if self._geom_ev is not None:
+            self._geom_ev.synchronize()          # the previous table upload has left the pinned block
+        C.memmove(self._geom_host.data_ptr(), C.addressof(rows), nb)
+        self._geom_dev[:nb].copy_(self._geom_host[:nb], non_blocking=True)
+        self._geom_ev = torch.cuda.Event()
+        self._geom_ev.record()
         c, ih, iw = self.model.INPUT_SHAPE
-        rc = self._lib.fm_roi_resize_norm_multi(ptr(self._frame_tab_dev), ptr(self._frame_idx_dev), w, h,
-                                                ptr(self._tlbr_dev), n, iw, ih, eng.inp_layout, ptr(eng.inp),
-                                                stream_ptr())
-        _lib.check(rc, "fm_roi_resize_norm_multi")
+        rc = self._lib.fm_roi_resize_norm_geom(ptr(self._geom_dev), ptr(self._frame_idx_dev), ptr(self._tlbr_dev), n,
+                                               iw, ih, eng.inp_layout, ptr(eng.inp), stream_ptr())
+        _lib.check(rc, "fm_roi_resize_norm_geom")
         self._out = eng.forward(n)
 
     def postprocess(self):

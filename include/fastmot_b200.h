@@ -161,6 +161,16 @@ typedef struct FmYoloHead {
     float scale_x_y;
 } FmYoloHead;
 
+/* One frame of a batch whose frames may differ in size: the device frame (BGR u8 HWC, w x h), its letterbox ROI in the
+ * network input, and the pixel scale (size_w, size_h = upscaled_sz) and offset (off_x, off_y = bbox_offset) the head
+ * decode maps its boxes back with -- the values a one-frame detector of that size passes as scalars. */
+typedef struct FmFrameGeom {
+    const unsigned char* frame;
+    int w, h;
+    int roi_x, roi_y, roi_w, roi_h;
+    float size_w, size_h, off_x, off_y;
+} FmFrameGeom;
+
 /* YOLODetector._preprocess + _create_letterbox (fastmot/detector.py:289-320): bilinear resize of the BGR u8 HWC
  * frame into the ROI [roi_x, roi_y, roi_w, roi_h] of a dst_w x dst_h network input (half-pixel centres, edge
  * replicate, rounded to u8 like the reference's CuPy zoom), BGR->RGB, x/255; everything outside the ROI = 0.5.
@@ -171,6 +181,10 @@ int fm_letterbox_preproc(const unsigned char* frame, int src_w, int src_h, int d
  * frame pointers; out is fp16 [batch][dst_h][dst_w][8], image b bit-identical to the one-frame call on frames[b]. */
 int fm_letterbox_preproc_batch(const unsigned char* const* frames, int batch, int src_w, int src_h, int dst_w,
                                int dst_h, int roi_x, int roi_y, int roi_w, int roi_h, void* out, void* stream);
+/* fm_letterbox_preproc (layout 1) of `batch` frames of any sizes in one launch: geom is a DEVICE array of batch rows
+ * (frame, w, h and roi_* are read; every roi_w, roi_h > 0); out is fp16 [batch][dst_h][dst_w][8], image b
+ * bit-identical to the one-frame call on geom[b]'s frame, size and ROI. */
+int fm_letterbox_preproc_geom(const FmFrameGeom* geom, int batch, int dst_w, int dst_h, void* out, void* stream);
 
 /* FeatureExtractor.extract_async preprocessing (fastmot/feature_extractor.py:48-60, 84-98; rect.py:92-97) for all
  * crops in one launch: integer-truncated clamp crop, OpenCV INTER_LINEAR 8-bit fixed-point resize to
@@ -185,6 +199,10 @@ int fm_roi_resize_norm(const unsigned char* frame, int src_w, int src_h, const d
  * bit-identical to the one-frame call on its own frame and box. */
 int fm_roi_resize_norm_multi(const unsigned char* const* frames, const int* frame_idx, int src_w, int src_h,
                              const double* tlbrs, int n, int out_w, int out_h, int layout, void* out, void* stream);
+/* fm_roi_resize_norm_multi over frames of any sizes: crop i is cut from geom[frame_idx[i]].frame, clamped to and
+ * addressed with that row's w and h (geom: DEVICE FmFrameGeom array; the ROI and scale fields are not read). */
+int fm_roi_resize_norm_geom(const FmFrameGeom* geom, const int* frame_idx, const double* tlbrs, int n, int out_w,
+                            int out_h, int layout, void* out, void* stream);
 
 /* CalDetection / CalDetection_NewCoords (fastmot/plugins/yolo_layer.cu:127-230) fused with the class mask +
  * score threshold + pixel scaling of YOLODetector._filter_dets (fastmot/detector.py:331-341).  One call per
@@ -206,6 +224,14 @@ int fm_yolo_decode_filter_batch(const void* head_out, int batch, long long head_
                                 const unsigned char* label_mask, double conf_thresh, float size_w, float size_h,
                                 float off_x, float off_y, float* dense, unsigned long long* keys, int* counters,
                                 int key_cap, void* stream);
+/* fm_yolo_decode_filter_batch with image b's size_w, size_h, off_x, off_y read from geom[b] (DEVICE FmFrameGeom array
+ * of batch rows): image b's keys and rows are the one-image call's on its head slice with its own geometry, in the
+ * segment layout fm_diou_nms_filter_batch reads. */
+int fm_yolo_decode_filter_geom(const void* head_out, int batch, long long head_stride, int is_fp16, int nhwc,
+                               int yolo_w, int yolo_h, int num_anchors, const FmYoloHead* h_head, int num_classes,
+                               int input_w, int input_h, int new_coords, int cand_base, int cand_stride,
+                               const unsigned char* label_mask, double conf_thresh, const FmFrameGeom* geom,
+                               float* dense, unsigned long long* keys, int* counters, int key_cap, void* stream);
 
 /* Rest of _filter_dets (detector.py:343-365) + diou_nms (rect.py:198-244): sort by (class, objectness desc),
  * per-class DIoU-NMS, to_tlbr rounding, area / aspect-ratio filters.  mask: >= fm_nms_mask_bytes(key_cap) bytes.
