@@ -48,7 +48,8 @@ class FmFlowPlan(C.Structure):
                 ("ransac_max_iter", c_i), ("ransac_conf", c_d), ("ransac_thresh", c_d), ("inlier_thresh", c_i),
                 ("refine_iters", c_i), ("good_idx", c_p), ("inl_idx", c_p), ("bg_kp", c_p), ("bg_kp_prev", c_p),
                 ("bg_kp_count", c_p), ("est_boxes", c_p), ("sig", c_p), ("klt_tlbr", c_p), ("klt_ok", c_p),
-                ("klt_ok_bytes", c_ll), ("inlier_ratio", c_p), ("rounds_ahead", c_i)]
+                ("klt_ok_bytes", c_ll), ("inlier_ratio", c_p), ("rounds_ahead", c_i),
+                ("block_size", c_i), ("gradient_size", c_i), ("use_harris", c_i), ("harris_k", c_d)]
 
 
 class FmConvDesc(C.Structure):
@@ -120,11 +121,14 @@ SIGNATURES = {
     "fm_yolo_decode_filter": (c_i, [c_p, c_i, c_i, c_i, c_i, c_i, C.POINTER(FmYoloHead), c_i, c_i, c_i, c_i, c_i, c_p,
                                      c_d, c_f, c_f, c_f, c_f, c_p, c_p, c_p, c_i, c_p]),
     "fm_gray_half": (c_i, [c_p, c_i, c_i, c_p, c_p, c_p]),
+    "fm_gray_resize": (c_i, [c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_p]),
     "fm_pyr_level": (c_i, [c_p, c_i, c_i, c_p, c_p]),
     "fm_scharr": (c_i, [c_p, c_i, c_i, c_p, c_p]),
     "fm_bg_small": (c_i, [c_p, c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_p]),
     "fm_flow_keypoints": (c_i, [c_p, c_i, c_i, c_p, c_p, c_i, c_p, c_p, c_p, c_i, c_d, c_d, c_d, c_i, c_p, c_p, c_i,
                                  c_p, c_p, c_p]),
+    "fm_flow_keypoints_cfg": (c_i, [c_p, c_i, c_i, c_p, c_p, c_i, c_p, c_p, c_p, c_i, c_d, c_d, c_d, c_i, c_i, c_i, c_i,
+                                     c_d, c_p, c_p, c_i, c_p, c_p, c_p]),
     "fm_fast_detect": (c_i, [c_p, c_p, c_i, c_i, c_i, c_f, c_f, c_p, c_p, c_p, c_i, c_p]),
     "fm_gather_points": (c_i, [c_p, c_p, c_i, c_p, c_i, c_p, c_p, c_p, c_p, c_p, c_i, c_p]),
     "fm_lk_track": (c_i, [c_p, c_p, c_p, c_p, c_f, c_f, c_i, c_i, c_i, c_f, c_f, c_f, c_p, c_p, c_p, c_p]),

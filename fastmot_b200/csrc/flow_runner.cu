@@ -117,13 +117,19 @@ extern "C" void fm_flow_plan_destroy(void* h) {
         }                                           \
     } while (0)
 
-// gray + 0.5x image + LK pyramid with Scharr derivatives for buffer k (flow.py:129-131 / :153-154)
+// gray + optical-flow image + LK pyramid with Scharr derivatives for buffer k (flow.py:129-131 / :153-154).  An
+// optical-flow image of exactly half the frame in both directions is the 2x2 mean (what cv2.resize computes there);
+// any other size is the general INTER_LINEAR resize.
 extern "C" int fm_flow_preprocess(void* h, const unsigned char* frame, int k, void* stream) {
     FlowRunner* r = (FlowRunner*)h;
     FM_REQUIRE(r && frame && (k == 0 || k == 1), "fm_flow_preprocess: bad handle / frame / buffer index");
     const FmFlowPlan& p = r->p;
     const FmPyramid& py = p.pyr[k];
-    FM_TRY(fm_gray_half(frame, p.frame_w, p.frame_h, p.gray[k], (unsigned char*)py.img[0], stream));
+    if (2 * py.w[0] == p.frame_w && 2 * py.h[0] == p.frame_h)
+        FM_TRY(fm_gray_half(frame, p.frame_w, p.frame_h, p.gray[k], (unsigned char*)py.img[0], stream));
+    else
+        FM_TRY(fm_gray_resize(frame, p.frame_w, p.frame_h, p.gray[k], (unsigned char*)py.img[0], py.w[0], py.h[0],
+                              stream));
     if (pyr_graph_enabled()) {
         if (r->pyr_state[k] == 0) build_pyr_graph(r, k);
         if (r->pyr_state[k] == 1) {
@@ -150,9 +156,10 @@ extern "C" int fm_flow_predict(void* h, const unsigned char* frame, int prev, in
     cudaStream_t sm = (cudaStream_t)s_main, ss = (cudaStream_t)s_side;
     FM_TRY(fm_flow_preprocess(h, frame, cur, s_main));
     FM_CUDA_TRY(cudaMemsetAsync(p.klt_ok, 0, (size_t)p.klt_ok_bytes, sm), "fm_flow_predict: klt_ok clear");
-    FM_TRY(fm_flow_keypoints(p.gray[prev], p.frame_w, p.frame_h, p.tlbr_pool, p.slots, n_trk, p.owner, p.kp_pool,
-                             p.kp_count, p.max_kp, p.feat_density, p.feat_dist_factor, p.quality, p.max_corners, p.jobs,
-                             p.scratch, p.scratch_cap, p.flags, p.flags + 1, s_main));
+    FM_TRY(fm_flow_keypoints_cfg(p.gray[prev], p.frame_w, p.frame_h, p.tlbr_pool, p.slots, n_trk, p.owner, p.kp_pool,
+                                 p.kp_count, p.max_kp, p.feat_density, p.feat_dist_factor, p.quality, p.max_corners,
+                                 p.block_size, p.gradient_size, p.use_harris, p.harris_k, p.jobs, p.scratch,
+                                 p.scratch_cap, p.flags, p.flags + 1, s_main));
     FM_TRY(fm_bg_small(p.gray[prev], p.owner, p.frame_w, p.frame_h, p.bg, p.bg_mask, p.bg_w, p.bg_h, s_main));
     FM_TRY(fm_fast_detect(p.bg, p.bg_mask, p.bg_w, p.bg_h, p.bg_thresh, p.unscale_x, p.unscale_y, p.bg_score, p.bg_pts,
                           p.bg_count, p.max_bg, s_main));

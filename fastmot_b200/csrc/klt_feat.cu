@@ -1,6 +1,10 @@
-// KLT keypoint maintenance: occlusion ("owner") map, per-track keypoint filtering, Shi-Tomasi re-detection
+// KLT keypoint maintenance: occlusion ("owner") map, per-track keypoint filtering, Shi-Tomasi / Harris re-detection
 // (cv2.goodFeaturesToTrack semantics) inside the visible part of each box, FAST-9/16 background corners,
 // and the gather that builds the flat point list for the LK kernel.
+//
+// goodFeaturesToTrack's default settings (blockSize 3, gradientSize 3, minimum eigenvalue, 0 < maxCorners <= 1024)
+// run gftt_eig_kernel and gftt_select_kernel<false>; every other setting runs gftt_response_kernel and
+// gftt_select_kernel<true>.
 //
 // Reference: fastmot/flow.py:156-200 (+ helpers :266-306, 335-344), fastmot/utils/rect.py:60-89,
 // fastmot/utils/numba.py:32-39.  OpenCV routines restated: goodFeaturesToTrack / cornerMinEigenVal
@@ -11,6 +15,9 @@
 // track k sees pixel p as foreground  <=>  owner[p] == k.
 #include "common.cuh"
 #include "../../include/fastmot_b200.h"
+
+#include <float.h>
+#include <limits.h>
 
 namespace {
 
@@ -59,7 +66,8 @@ __global__ void __launch_bounds__(256) kp_prepare_kernel(const double* __restric
                                                           const int* __restrict__ owner, float* __restrict__ kp_pool,
                                                           int* __restrict__ kp_count, int max_kp, double feat_density,
                                                           double feat_dist_factor, FmTrackJob* __restrict__ jobs,
-                                                          int* __restrict__ scratch_counter, int scratch_cap) {
+                                                          int* __restrict__ scratch_counter, int scratch_cap,
+                                                          int scratch_per_px) {
     __shared__ int s_cnt[8];
     __shared__ int s_area, s_base, s_total;
     const int k = blockIdx.x;
@@ -134,7 +142,7 @@ __global__ void __launch_bounds__(256) kp_prepare_kernel(const double* __restric
         job.scratch_off = -1;
         job.eig_max = 0.f;
         if (job.redetect) {
-            int need = job.cw * job.ch;
+            int need = job.cw * job.ch * scratch_per_px;
             int off = atomicAdd(scratch_counter, need);
             if (off + need <= scratch_cap) job.scratch_off = off;
             else job.redetect = 2;  // overflow flag, surfaced to the host
@@ -147,7 +155,8 @@ __global__ void __launch_bounds__(256) kp_prepare_kernel(const double* __restric
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// cornerMinEigenVal(blockSize 3, Sobel 3) on the crop of the previous gray frame; reflect-101 on the crop.
+// The default setting: cornerMinEigenVal(blockSize 3, Sobel 3) on the crop of the previous gray frame; reflect-101 on
+// the crop.
 // ---------------------------------------------------------------------------------------------------------
 __device__ __forceinline__ int refl(int p, int n) {
     if (n == 1) return 0;
@@ -202,19 +211,115 @@ __global__ void __launch_bounds__(256) gftt_eig_kernel(const unsigned char* __re
     }
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// cornerMinEigenVal / cornerHarris (corner.cpp: cornerEigenValsVecs) for any blockSize >= 1 and Sobel aperture
+// 1 / 3 / 5 / 7 on the crop of the previous gray frame; reflect-101 on the crop for the Sobel and the box filter.
+// Pass 1 writes the scaled gradient products (Dx^2, Dx*Dy, Dy^2) of every crop pixel to three scratch planes after
+// the response map, pass 2 sums them over the unnormalised blockSize x blockSize window anchored at blockSize / 2
+// (even sizes reach one pixel further up / left) and forms the response.  The selection only needs the corners it
+// picks to be OpenCV's, not the response bits: the float sums run in a different order than OpenCV's filters.
+// ---------------------------------------------------------------------------------------------------------
+// Sobel taps of aperture 1 / 3 / 5 / 7 centred in 7 entries: smoothing (binomial) and first derivative.
+// Aperture 1 is the 3-tap [-1 0 1] derivative with no smoothing (getSobelKernels).
+__constant__ int c_sobel_smooth[4][7] = {{0, 0, 0, 1, 0, 0, 0}, {0, 0, 1, 2, 1, 0, 0}, {0, 1, 4, 6, 4, 1, 0},
+                                         {1, 6, 15, 20, 15, 6, 1}};
+__constant__ int c_sobel_deriv[4][7] = {{0, 0, -1, 0, 1, 0, 0}, {0, 0, -1, 0, 1, 0, 0}, {0, -1, -2, 0, 2, 1, 0},
+                                        {-1, -4, -5, 0, 5, 4, 1}};
+
+__global__ void __launch_bounds__(256) gftt_response_kernel(const unsigned char* __restrict__ gray, int w, int h,
+                                                             const int* __restrict__ owner,
+                                                             FmTrackJob* __restrict__ jobs, int n_trk,
+                                                             float* __restrict__ scratch, int block_size,
+                                                             int gradient_size, int use_harris, float harris_k) {
+    __shared__ float s_max[8];
+    const int k = blockIdx.x;
+    if (k >= n_trk) return;
+    const FmTrackJob job = jobs[k];
+    if (job.redetect != 1) return;
+    const int cw = job.cw, ch = job.ch, n = cw * ch;
+    const int t = gradient_size >> 1, r = gradient_size == 1 ? 1 : t;   // table row, tap radius
+    const float scale = (float)(1.0 / ((double)(1 << (gradient_size - 1)) * block_size * 255.0));
+    float* eig = scratch + job.scratch_off;
+    float* cxx = eig + n;
+    float* cxy = cxx + n;
+    float* cyy = cxy + n;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const int y = i / cw, x = i - y * cw;
+        int cols[7];
+        for (int q = -r; q <= r; ++q) cols[q + 3] = job.x0 + refl(x + q, cw);
+        int gx = 0, gy = 0;
+        for (int p = -r; p <= r; ++p) {
+            const unsigned char* row = gray + (size_t)(job.y0 + refl(y + p, ch)) * w;
+            int dxr = 0, sxr = 0;
+            for (int q = -r; q <= r; ++q) {
+                const int v = row[cols[q + 3]];
+                dxr += c_sobel_deriv[t][q + 3] * v;
+                sxr += c_sobel_smooth[t][q + 3] * v;
+            }
+            gx += c_sobel_smooth[t][p + 3] * dxr;
+            gy += c_sobel_deriv[t][p + 3] * sxr;
+        }
+        const float fx = gx * scale, fy = gy * scale;
+        cxx[i] = fx * fx; cxy[i] = fx * fy; cyy[i] = fy * fy;
+    }
+    __syncthreads();
+    const int anchor = block_size >> 1;
+    float vmax = -FLT_MAX;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const int y = i / cw, x = i - y * cw;
+        float a = 0.f, b = 0.f, c = 0.f;
+        for (int p = 0; p < block_size; ++p) {
+            const int ro = refl(y - anchor + p, ch) * cw;
+            for (int q = 0; q < block_size; ++q) {
+                const int j = ro + refl(x - anchor + q, cw);
+                a += cxx[j]; b += cxy[j]; c += cyy[j];
+            }
+        }
+        float v;
+        if (use_harris) {
+            v = a * c - b * b - harris_k * (a + c) * (a + c);
+        } else {
+            a *= 0.5f; c *= 0.5f;
+            v = (a + c) - sqrtf((a - c) * (a - c) + b * b);
+        }
+        eig[i] = v;
+        if (owner[(size_t)(job.y0 + y) * w + job.x0 + x] == k) vmax = fmaxf(vmax, v);
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) vmax = fmaxf(vmax, __shfl_xor_sync(0xffffffffu, vmax, o));
+    if ((threadIdx.x & 31) == 0) s_max[threadIdx.x >> 5] = vmax;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float m = -FLT_MAX;
+        for (int i = 0; i < (int)(blockDim.x >> 5); ++i) m = fmaxf(m, s_max[i]);
+        jobs[k].eig_max = m == -FLT_MAX ? 0.f : m;      // minMaxLoc over an empty mask gives 0
+    }
+}
+
+// Ascending order of the key == descending order of v, for either sign (the Harris response can be negative).
+__device__ __forceinline__ unsigned desc_key(float v) {
+    const unsigned u = __float_as_uint(v);
+    return (u & 0x80000000u) ? u : ~(u | 0x80000000u);
+}
+
 // threshold + 3x3 local maximum + sort (value desc, address desc) + greedy min-distance + ellipse filter.
+// kGeneral = false: the default settings (response > 0, at most 1024 corners kept in shared memory).  kGeneral = true:
+// any response sign (THRESH_TOZERO is applied to the neighbours before the local-maximum test, as OpenCV's dilate
+// sees them), maxCorners <= 0 means no limit, and the accepted corners go to acc_list (two ints per corner, in the
+// gradient planes of this track's scratch, free once the response is final).
 #define GFTT_MAX_CAND 4096
+template <bool kGeneral>
 __global__ void __launch_bounds__(256) gftt_select_kernel(const int* __restrict__ owner, int w, int h,
                                                            const double* __restrict__ tlbr_pool,
                                                            FmTrackJob* __restrict__ jobs, int n_trk,
                                                            const float* __restrict__ scratch, double quality,
                                                            int max_corners, float* __restrict__ kp_pool,
                                                            int* __restrict__ kp_count, int max_kp,
-                                                           int* __restrict__ status) {
+                                                           int* __restrict__ status, float* __restrict__ acc_scratch) {
     __shared__ unsigned long long s_key[GFTT_MAX_CAND];
     __shared__ unsigned char s_dead[GFTT_MAX_CAND];
     __shared__ int s_n, s_nacc, s_cur;
-    __shared__ short s_accx[1024], s_accy[1024];
+    __shared__ short s_accx[kGeneral ? 1 : 1024], s_accy[kGeneral ? 1 : 1024];
     const int k = blockIdx.x;
     if (k >= n_trk) return;
     const FmTrackJob job = jobs[k];
@@ -222,6 +327,7 @@ __global__ void __launch_bounds__(256) gftt_select_kernel(const int* __restrict_
     if (job.redetect != 1) return;
     const int cw = job.cw, ch = job.ch, tid = threadIdx.x;
     const float* eig = scratch + job.scratch_off;
+    int* acc_list = kGeneral ? (int*)(acc_scratch + job.scratch_off + cw * ch) : nullptr;
     const float thr = (float)((double)job.eig_max * quality);
     if (tid == 0) { s_n = 0; s_nacc = 0; }
     __syncthreads();
@@ -230,17 +336,23 @@ __global__ void __launch_bounds__(256) gftt_select_kernel(const int* __restrict_
         if (y < 1 || x < 1 || y >= ch - 1 || x >= cw - 1) continue;
         const float v = eig[i];
         if (!(v > thr)) continue;  // THRESH_TOZERO then `val != 0`
+        if (kGeneral && v == 0.f) continue;
         if (owner[(size_t)(job.y0 + y) * w + job.x0 + x] != k) continue;
         bool ismax = true;
 #pragma unroll
         for (int dy = -1; dy <= 1; ++dy)
 #pragma unroll
-            for (int dx = -1; dx <= 1; ++dx) ismax = ismax && (v >= eig[(y + dy) * cw + (x + dx)]);
+            for (int dx = -1; dx <= 1; ++dx) {
+                float nb = eig[(y + dy) * cw + (x + dx)];
+                if (kGeneral && !(nb > thr)) nb = 0.f;
+                ismax = ismax && (v >= nb);
+            }
         if (!ismax) continue;
         const int pos = atomicAdd(&s_n, 1);
         if (pos < GFTT_MAX_CAND) {
             // ascending u64 sort == value desc (v > 0), then pixel index desc
-            s_key[pos] = ((unsigned long long)(~__float_as_uint(v)) << 32) | (unsigned)(0x7fffffff - i);
+            const unsigned vk = kGeneral ? desc_key(v) : ~__float_as_uint(v);
+            s_key[pos] = ((unsigned long long)vk << 32) | (unsigned)(0x7fffffff - i);
         }
     }
     __syncthreads();
@@ -268,7 +380,7 @@ __global__ void __launch_bounds__(256) gftt_select_kernel(const int* __restrict_
     // greedy min-distance: one barrier pair per ACCEPTED corner
     const int md2 = job.min_dist * job.min_dist;
     int cur = 0;
-    const int cap = min(max_corners, 1024);
+    const int cap = kGeneral ? (max_corners > 0 ? max_corners : INT_MAX) : min(max_corners, 1024);
     while (true) {
         if (tid == 0) {
             int c = cur;
@@ -280,7 +392,11 @@ __global__ void __launch_bounds__(256) gftt_select_kernel(const int* __restrict_
         if (cur >= n) break;
         const int idx = 0x7fffffff - (int)(s_key[cur] & 0xffffffffu);
         const int cy = idx / cw, cx = idx - cy * cw;
-        if (tid == 0) { s_accx[s_nacc] = cx; s_accy[s_nacc] = cy; s_nacc = s_nacc + 1; }
+        if (tid == 0) {
+            if (kGeneral) { acc_list[2 * s_nacc] = cx; acc_list[2 * s_nacc + 1] = cy; }
+            else { s_accx[s_nacc] = cx; s_accy[s_nacc] = cy; }
+            s_nacc = s_nacc + 1;
+        }
         for (int j = cur + 1 + tid; j < n; j += blockDim.x) {
             if (s_dead[j]) continue;
             const int ji = 0x7fffffff - (int)(s_key[j] & 0xffffffffu);
@@ -300,7 +416,8 @@ __global__ void __launch_bounds__(256) gftt_select_kernel(const int* __restrict_
         float* kp = kp_pool + (size_t)job.slot * max_kp * 2;
         int m = 0;
         for (int i = 0; i < s_nacc && m < max_kp; ++i) {
-            const float px = (float)s_accx[i] + (float)job.x0, py = (float)s_accy[i] + (float)job.y0;
+            const int ax_i = kGeneral ? acc_list[2 * i] : s_accx[i], ay_i = kGeneral ? acc_list[2 * i + 1] : s_accy[i];
+            const float px = (float)ax_i + (float)job.x0, py = (float)ay_i + (float)job.y0;
             const double ux = ((double)px - ccx) / ax, uy = ((double)py - ccy) / ay;
             if (ux * ux + uy * uy <= 1.0) { kp[2 * m] = px; kp[2 * m + 1] = py; ++m; }
         }
@@ -492,12 +609,45 @@ extern "C" int fm_flow_keypoints(const unsigned char* prev_gray, int w, int h, c
     if (n_trk > 0) {
         owner_paint_kernel<<<n_trk, 256, 0, s>>>(tlbr_pool, slots, n_trk, w, h, owner);
         kp_prepare_kernel<<<n_trk, 256, 0, s>>>(tlbr_pool, slots, n_trk, w, h, owner, kp_pool, kp_count, max_kp,
-                                                feat_density, feat_dist_factor, jobs, scratch_counter, scratch_cap);
+                                                feat_density, feat_dist_factor, jobs, scratch_counter, scratch_cap, 1);
         gftt_eig_kernel<<<n_trk, 256, 0, s>>>(prev_gray, w, h, owner, jobs, n_trk, scratch);
-        gftt_select_kernel<<<n_trk, 256, 0, s>>>(owner, w, h, tlbr_pool, jobs, n_trk, scratch, quality, max_corners,
-                                                 kp_pool, kp_count, max_kp, status);
+        gftt_select_kernel<false><<<n_trk, 256, 0, s>>>(owner, w, h, tlbr_pool, jobs, n_trk, scratch, quality,
+                                                        max_corners, kp_pool, kp_count, max_kp, status, nullptr);
     }
     FM_CHECK_LAUNCH("fm_flow_keypoints");
+    return FM_OK;
+}
+
+extern "C" int fm_flow_keypoints_cfg(const unsigned char* prev_gray, int w, int h, const double* tlbr_pool,
+                                     const int* slots, int n_trk, int* owner, float* kp_pool, int* kp_count,
+                                     int max_kp, double feat_density, double feat_dist_factor, double quality,
+                                     int max_corners, int block_size, int gradient_size, int use_harris,
+                                     double harris_k, FmTrackJob* jobs, float* scratch, int scratch_cap,
+                                     int* scratch_counter, int* status, void* stream) {
+    if (block_size == 3 && gradient_size == 3 && !use_harris && max_corners > 0 && max_corners <= 1024)
+        return fm_flow_keypoints(prev_gray, w, h, tlbr_pool, slots, n_trk, owner, kp_pool, kp_count, max_kp,
+                                 feat_density, feat_dist_factor, quality, max_corners, jobs, scratch, scratch_cap,
+                                 scratch_counter, status, stream);
+    FM_REQUIRE(block_size >= 1, "fm_flow_keypoints_cfg: blockSize must be >= 1");
+    FM_REQUIRE(gradient_size == 1 || gradient_size == 3 || gradient_size == 5 || gradient_size == 7,
+               "fm_flow_keypoints_cfg: gradientSize must be 1, 3, 5 or 7");
+    FM_REQUIRE(max_kp >= (max_corners > 0 ? min(max_corners, GFTT_MAX_CAND) : GFTT_MAX_CAND),
+               "fm_flow_keypoints_cfg: max_kp is smaller than the corners one track may keep");
+    cudaStream_t s = (cudaStream_t)stream;
+    owner_clear_kernel<<<FM_NUM_SMS * 4, 256, 0, s>>>(owner, (size_t)w * h);
+    cudaMemsetAsync(scratch_counter, 0, sizeof(int), s);
+    cudaMemsetAsync(status, 0, sizeof(int), s);
+    if (n_trk > 0) {
+        owner_paint_kernel<<<n_trk, 256, 0, s>>>(tlbr_pool, slots, n_trk, w, h, owner);
+        // four floats per crop pixel: the response map and the three gradient-product planes
+        kp_prepare_kernel<<<n_trk, 256, 0, s>>>(tlbr_pool, slots, n_trk, w, h, owner, kp_pool, kp_count, max_kp,
+                                                feat_density, feat_dist_factor, jobs, scratch_counter, scratch_cap, 4);
+        gftt_response_kernel<<<n_trk, 256, 0, s>>>(prev_gray, w, h, owner, jobs, n_trk, scratch, block_size,
+                                                   gradient_size, use_harris, (float)harris_k);
+        gftt_select_kernel<true><<<n_trk, 256, 0, s>>>(owner, w, h, tlbr_pool, jobs, n_trk, scratch, quality,
+                                                       max_corners, kp_pool, kp_count, max_kp, status, scratch);
+    }
+    FM_CHECK_LAUNCH("fm_flow_keypoints_cfg");
     return FM_OK;
 }
 

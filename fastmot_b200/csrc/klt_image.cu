@@ -1,5 +1,6 @@
-// KLT image pyramid kernels (byte work, HBM/L2-bound): BGR->gray + 0.5x box mean in one pass, 5-tap Gaussian
-// pyrDown, int16 Scharr derivatives, 0.1x background image + mask.
+// KLT image pyramid kernels (byte work, HBM/L2-bound): BGR->gray + 0.5x box mean in one pass, BGR->gray + an
+// INTER_LINEAR resize to any optical-flow size, 5-tap Gaussian pyrDown, int16 Scharr derivatives, 0.1x background
+// image + mask.
 //
 // Reference: fastmot/flow.py:121-133, 153-154, 187-189 (cv2.cvtColor / cv2.resize) and the pyramid that
 // cv2.calcOpticalFlowPyrLK builds internally (flow.py:203-207; OpenCV lkpyramid.cpp: buildOpticalFlowPyramid,
@@ -33,6 +34,39 @@ __global__ void __launch_bounds__(256) gray_half_kernel(const unsigned char* __r
     gray[(size_t)y1 * w + x0] = c;
     gray[(size_t)y1 * w + x1] = d;
     small[(size_t)y * sw + x] = (a + b + c + d + 2) >> 2;  // cv2.resize INTER_LINEAR at exactly 0.5x
+}
+
+__global__ void __launch_bounds__(256) gray_kernel(const unsigned char* __restrict__ frame, int w, int h,
+                                                    unsigned char* __restrict__ gray) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    const int y = blockIdx.y;
+    if (x >= w || y >= h) return;
+    gray[(size_t)y * w + x] = gray_of(frame + ((size_t)y * w + x) * 3);
+}
+
+// cv2.resize(src, (dw, dh)) INTER_LINEAR for u8 at a downscale (dw <= sw, dh <= sh): OpenCV's generic resize with
+// 11-bit coefficients (resize.cpp: scale = 1 / (dsize / ssize), coefficients rounded half to even, the vertical pass
+// of VResizeLinearVec_32s8u).  The source rows / columns are clamped at the far edge, where the weight is zero.
+__global__ void __launch_bounds__(256) resize_linear_kernel(const unsigned char* __restrict__ src, int sw, int sh,
+                                                             unsigned char* __restrict__ dst, int dw, int dh,
+                                                             double scale_x, double scale_y) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    const int y = blockIdx.y;
+    if (x >= dw || y >= dh) return;
+    float fx = (float)((x + 0.5) * scale_x - 0.5), fy = (float)((y + 0.5) * scale_y - 0.5);
+    int sx = (int)floorf(fx), sy = (int)floorf(fy);
+    fx -= sx; fy -= sy;
+    if (sx < 0) { fx = 0; sx = 0; }
+    if (sx >= sw - 1) { fx = 0; sx = sw - 1; }
+    if (sy < 0) { fy = 0; sy = 0; }
+    if (sy >= sh - 1) { fy = 0; sy = sh - 1; }
+    const int a0 = (int)rintf((1.f - fx) * 2048.f), a1 = (int)rintf(fx * 2048.f);
+    const int b0 = (int)rintf((1.f - fy) * 2048.f), b1 = (int)rintf(fy * 2048.f);
+    const int sx1 = min(sx + 1, sw - 1), sy1 = min(sy + 1, sh - 1);
+    const unsigned char* r0 = src + (size_t)sy * sw;
+    const unsigned char* r1 = src + (size_t)sy1 * sw;
+    const int h0 = r0[sx] * a0 + r0[sx1] * a1, h1 = r1[sx] * a0 + r1[sx1] * a1;
+    dst[(size_t)y * dw + x] = (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2;
 }
 
 __device__ __forceinline__ int reflect101(int p, int n) {
@@ -111,6 +145,18 @@ extern "C" int fm_gray_half(const unsigned char* frame, int w, int h, unsigned c
     dim3 grid(fm_cdiv(sw, 256), sh);
     gray_half_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(frame, w, h, gray, small, sw, sh);
     FM_CHECK_LAUNCH("fm_gray_half");
+    return FM_OK;
+}
+
+extern "C" int fm_gray_resize(const unsigned char* frame, int w, int h, unsigned char* gray, unsigned char* small,
+                              int sw, int sh, void* stream) {
+    FM_REQUIRE(w > 0 && h > 0 && sw > 0 && sh > 0 && sw <= w && sh <= h,
+               "fm_gray_resize: the optical-flow image must be non-empty and no larger than the frame");
+    gray_kernel<<<dim3(fm_cdiv(w, 256), h), 256, 0, (cudaStream_t)stream>>>(frame, w, h, gray);
+    resize_linear_kernel<<<dim3(fm_cdiv(sw, 256), sh), 256, 0, (cudaStream_t)stream>>>(
+        gray, w, h, small, sw, sh, 1.0 / ((double)sw / w), 1.0 / ((double)sh / h));
+    fm_count_launches(1);
+    FM_CHECK_LAUNCH("fm_gray_resize");
     return FM_OK;
 }
 

@@ -352,7 +352,10 @@ __device__ __forceinline__ bool affine_inlier(const double* F, const float* f, c
 #define AFF_MAX_PTS 1024
 #define AFF_BATCH 32
 
-// One CTA (128 threads) per track per round.
+// One CTA (128 threads) per track per round.  kMaxPts bounds the points of one track: AFF_MAX_PTS when a track keeps
+// at most 1024 keypoints (goodFeaturesToTrack's default settings), AFF_MAX_PTS_LARGE when maxCorners allows more.
+#define AFF_MAX_PTS_LARGE 4096
+template <int kMaxPts>
 __global__ void __launch_bounds__(128) affine_partial_kernel(
     const float* __restrict__ all_prev, const float* __restrict__ all_cur, const unsigned char* __restrict__ status,
     const int* __restrict__ trk_begin, const int* __restrict__ slots, int n_trk, int round,
@@ -362,8 +365,8 @@ __global__ void __launch_bounds__(128) affine_partial_kernel(
     unsigned char* __restrict__ klt_ok, double* __restrict__ inlier_ratio, float* __restrict__ kp_pool,
     float* __restrict__ kp_prev_pool, int* __restrict__ kp_count, int max_kp, int frame_w, int frame_h, int max_iters,
     double confidence, double thresh, int inlier_thresh, int refine_iters) {
-    __shared__ int s_idx[AFF_MAX_PTS];
-    __shared__ int s_inl[AFF_MAX_PTS];
+    __shared__ int s_idx[kMaxPts];
+    __shared__ int s_inl[kMaxPts];
     __shared__ int s_sub[AFF_BATCH][2];
     __shared__ double s_model[AFF_BATCH][6];
     __shared__ int s_cnt[AFF_BATCH];
@@ -398,9 +401,9 @@ __global__ void __launch_bounds__(128) affine_partial_kernel(
         int off = s_n;
         for (int w = 0; w < wid; ++w) off += s_warpcnt[w];
         off += __popc(bal & ((1u << lane) - 1));
-        if (keep && off < AFF_MAX_PTS) s_idx[off] = i;
+        if (keep && off < kMaxPts) s_idx[off] = i;
         __syncthreads();
-        if (tid == 0) s_n = min(s_n + s_warpcnt[0] + s_warpcnt[1] + s_warpcnt[2] + s_warpcnt[3], AFF_MAX_PTS);
+        if (tid == 0) s_n = min(s_n + s_warpcnt[0] + s_warpcnt[1] + s_warpcnt[2] + s_warpcnt[3], kMaxPts);
         __syncthreads();
     }
     const int m = s_n;
@@ -1016,7 +1019,9 @@ extern "C" int fm_ransac_affine_partial_batch(const float* all_prev, const float
                                               int max_iters, double confidence, double thresh, int inlier_thresh,
                                               int refine_iters, int first_round, void* stream) {
     if (n_trk <= 0) return FM_OK;
+    FM_REQUIRE(max_kp <= AFF_MAX_PTS_LARGE, "fm_ransac_affine_partial_batch: max_kp above 4096");
     cudaStream_t s = (cudaStream_t)stream;
+    auto kernel = max_kp <= AFF_MAX_PTS ? affine_partial_kernel<AFF_MAX_PTS> : affine_partial_kernel<AFF_MAX_PTS_LARGE>;
     for (int r = first_round; r < first_round + n_rounds; ++r) {
         const int* prev_flag = r > 0 ? round_flags + ((r - 1) & 15) : nullptr;
         int* cur_flag = round_flags + (r & 15);
@@ -1024,10 +1029,10 @@ extern "C" int fm_ransac_affine_partial_batch(const float* all_prev, const float
         const int* est_prev = est_boxes + ((r + 1) & 1) * n_trk * 5;
         int* est_cur = est_boxes + (r & 1) * n_trk * 5;
         if (r == 0) cudaMemsetAsync(est_boxes, 0, sizeof(int) * 2 * n_trk * 5, s);
-        affine_partial_kernel<<<n_trk, 128, 0, s>>>(all_prev, all_cur, status, trk_begin, slots, n_trk, r, prev_flag,
-                                                    cur_flag, h_ok, est_prev, est_cur, sig, tlbr_pool, klt_tlbr, klt_ok,
-                                                    inlier_ratio, kp_pool, kp_prev_pool, kp_count, max_kp, frame_w,
-                                                    frame_h, max_iters, confidence, thresh, inlier_thresh, refine_iters);
+        kernel<<<n_trk, 128, 0, s>>>(all_prev, all_cur, status, trk_begin, slots, n_trk, r, prev_flag, cur_flag, h_ok,
+                                     est_prev, est_cur, sig, tlbr_pool, klt_tlbr, klt_ok, inlier_ratio, kp_pool,
+                                     kp_prev_pool, kp_count, max_kp, frame_w, frame_h, max_iters, confidence, thresh,
+                                     inlier_thresh, refine_iters);
     }
     FM_CHECK_LAUNCH("fm_ransac_affine_partial_batch");
     return FM_OK;

@@ -1,7 +1,8 @@
 """KLT optical-flow stage on the GPU with the reference's constructor / attributes (fastmot/flow.py:16-264).
 
-`predict_device` enqueues the whole of `Flow.predict` — gray + 0.5x pyramid with Scharr derivatives, occlusion
-("owner") map, per-track keypoint filtering and Shi-Tomasi re-detection, FAST background corners, pyramidal LK on
+`predict_device` enqueues the whole of `Flow.predict` — gray + optical-flow image (any frame size and scale) and its
+pyramid with Scharr derivatives, occlusion ("owner") map, per-track keypoint filtering and Shi-Tomasi / Harris
+re-detection (every cv2.goodFeaturesToTrack setting), FAST background corners, pyramidal LK on
 all points at once, RANSAC homography, per-track RANSAC partial-affine with box prediction — as ~15 kernel
 launches with no OpenCV and no host round trip except one 16-byte status read.  Results stay on the device:
 predicted boxes / flags / inlier ratios in the track pool, the homography in a 9-double buffer that the batched
@@ -18,6 +19,11 @@ from . import _lib
 from .devmem import ptr, stream_ptr, FrameUploader
 
 LOGGER = logging.getLogger(__name__)
+
+# candidate corners one box may hold in the selection kernel (csrc/klt_feat.cu GFTT_MAX_CAND); more raise at run time
+GFTT_MAX_CAND = 4096
+# keyword arguments of cv2.goodFeaturesToTrack that obj_feat_params may set (minDistance and mask come from the track)
+_GFTT_KEYS = {"maxCorners", "qualityLevel", "blockSize", "useHarrisDetector", "k", "gradientSize"}
 
 
 def _depth_key(track):
@@ -68,17 +74,42 @@ class Flow:
         self.opt_flow_params = {"winSize": (5, 5), "maxLevel": 5, "criteria": (3, 10, 0.03)}
         if obj_feat_params is not None:
             self.obj_feat_params.update(vars(obj_feat_params))
-        if self.obj_feat_params["blockSize"] != 3:
-            raise NotImplementedError("Shi-Tomasi kernel is written for blockSize 3 (the reference default)")
-        if tuple(opt_flow_scale_factor) != (0.5, 0.5) or size[0] % 2 or size[1] % 2:
-            raise NotImplementedError("optical-flow scale must be 0.5 on an even frame size (2x2 mean kernel)")
+        unknown = set(self.obj_feat_params) - _GFTT_KEYS
+        if unknown:
+            raise TypeError(f"obj_feat_params: cv2.goodFeaturesToTrack takes no argument {sorted(unknown)}")
+        mk = self.obj_feat_params
+        self.block_size = int(mk["blockSize"])
+        self.gradient_size = int(mk.get("gradientSize", 3))
+        self.use_harris = bool(mk.get("useHarrisDetector", False))
+        self.harris_k = float(mk.get("k", 0.04))
+        if self.block_size < 1:
+            raise ValueError(f"obj_feat_params.blockSize must be >= 1, got {mk['blockSize']}")
+        if self.gradient_size not in (1, 3, 5, 7):
+            raise ValueError(f"obj_feat_params.gradientSize must be 1, 3, 5 or 7, got {mk.get('gradientSize')}")
+        # the default goodFeaturesToTrack setting runs the original kernels (csrc/klt_feat.cu)
+        self._default_feat = (self.block_size == 3 and self.gradient_size == 3 and not self.use_harris
+                              and 0 < int(mk["maxCorners"]) <= 1024)
+        # keypoint rows per track (TrackPool.max_kp): 1024 up to maxCorners 1024, else maxCorners bounded by the
+        # candidate cap (maxCorners <= 0 is no limit)
+        mc = int(mk["maxCorners"])
+        self.max_kp = 1024 if 0 < mc <= 1024 else min(mc if mc > 0 else GFTT_MAX_CAND, GFTT_MAX_CAND)
 
-        self._lib = _lib.require_device()
         W, H = size
-        dev = torch.device("cuda")
-        u8, i32, f32 = torch.uint8, torch.int32, torch.float32
+        # Python's round (half to even), as the reference sizes its buffers (flow.py:102-105)
         self.opt_flow_sz = (round(opt_flow_scale_factor[0] * W), round(opt_flow_scale_factor[1] * H))
         self.bg_feat_sz = (round(bg_feat_scale_factor[0] * W), round(bg_feat_scale_factor[1] * H))
+        if min(self.opt_flow_sz) < 1:
+            raise ValueError(f"opt_flow_scale_factor {tuple(opt_flow_scale_factor)} gives an empty optical-flow image "
+                             f"{self.opt_flow_sz} for frame size {tuple(size)}")
+        if min(self.bg_feat_sz) < 1:
+            raise ValueError(f"bg_feat_scale_factor {tuple(bg_feat_scale_factor)} gives an empty background image "
+                             f"{self.bg_feat_sz} for frame size {tuple(size)}")
+        # exactly half the frame both ways: cv2.resize's 2x2 mean (fm_gray_half); otherwise INTER_LINEAR (fm_gray_resize)
+        self._half = 2 * self.opt_flow_sz[0] == W and 2 * self.opt_flow_sz[1] == H
+
+        self._lib = _lib.require_device()
+        dev = torch.device("cuda")
+        u8, i32, f32 = torch.uint8, torch.int32, torch.float32
         win_w, win_h = self.opt_flow_params["winSize"]
         # pyramid geometry of cv::buildOpticalFlowPyramid
         sizes = [self.opt_flow_sz]
@@ -145,6 +176,9 @@ class Flow:
         self.rounds_last = 0
 
     def bind_pool(self, pool):
+        if pool.max_kp < self.max_kp:
+            raise ValueError(f"TrackPool.max_kp {pool.max_kp} < {self.max_kp} keypoints per track that maxCorners "
+                             f"{self.obj_feat_params['maxCorners']} allows")
         if getattr(self, "_runner", None) is not None:
             self._lib.fm_flow_plan_destroy(self._runner)
         self.pool = pool
@@ -193,6 +227,8 @@ class Flow:
         P.klt_ok_bytes = pool.klt_ok.numel() * pool.klt_ok.element_size()
         P.inlier_ratio = pool.inlier_ratio.data_ptr()
         P.rounds_ahead = self.ROUNDS_AHEAD
+        P.block_size, P.gradient_size = self.block_size, self.gradient_size
+        P.use_harris, P.harris_k = int(self.use_harris), self.harris_k
         return P
 
     def _get_runner(self):
@@ -238,11 +274,17 @@ class Flow:
         return frame if torch.is_tensor(frame) else self._uploader.upload(frame)
 
     def _preprocess(self, frame_dev, k):
-        """cvtColor + 0.5x resize (flow.py:153-154) and the LK pyramid with derivatives for buffer k."""
+        """cvtColor + resize (flow.py:153-154) and the LK pyramid with derivatives for buffer k."""
         W, H = self.size
         s = stream_ptr()
         lib = self._lib
-        _lib.check(lib.fm_gray_half(ptr(frame_dev), W, H, ptr(self.gray[k]), ptr(self.pyr[k][0]), s), "fm_gray_half")
+        if self._half:
+            _lib.check(lib.fm_gray_half(ptr(frame_dev), W, H, ptr(self.gray[k]), ptr(self.pyr[k][0]), s),
+                       "fm_gray_half")
+        else:
+            sw, sh = self.opt_flow_sz
+            _lib.check(lib.fm_gray_resize(ptr(frame_dev), W, H, ptr(self.gray[k]), ptr(self.pyr[k][0]), sw, sh, s),
+                       "fm_gray_resize")
         for i, (w, h) in enumerate(self.level_sizes):
             if i + 1 < len(self.level_sizes):
                 _lib.check(lib.fm_pyr_level(ptr(self.pyr[k][i]), w, h, ptr(self.pyr[k][i + 1]), s), "fm_pyr_level")
@@ -292,12 +334,20 @@ class Flow:
         pool.klt_ok.zero_()
         fl = self.flags.data_ptr()
         mk = self.obj_feat_params
-        _lib.check(lib.fm_flow_keypoints(ptr(self.gray[self.prev]), W, H, ptr(pool.tlbr), ptr(self.slots_dev), n,
-                                         ptr(self.owner), ptr(pool.kp), ptr(pool.kp_count), pool.max_kp,
-                                         float(self.feat_density), float(self.feat_dist_factor),
-                                         float(mk["qualityLevel"]), int(mk["maxCorners"]), ptr(self.jobs),
-                                         ptr(self.scratch), self.scratch_cap, C.c_void_p(fl), C.c_void_p(fl + 4), s),
-                   "fm_flow_keypoints")
+        if self._default_feat:
+            _lib.check(lib.fm_flow_keypoints(ptr(self.gray[self.prev]), W, H, ptr(pool.tlbr), ptr(self.slots_dev), n,
+                                             ptr(self.owner), ptr(pool.kp), ptr(pool.kp_count), pool.max_kp,
+                                             float(self.feat_density), float(self.feat_dist_factor),
+                                             float(mk["qualityLevel"]), int(mk["maxCorners"]), ptr(self.jobs),
+                                             ptr(self.scratch), self.scratch_cap, C.c_void_p(fl), C.c_void_p(fl + 4),
+                                             s), "fm_flow_keypoints")
+        else:
+            _lib.check(lib.fm_flow_keypoints_cfg(
+                ptr(self.gray[self.prev]), W, H, ptr(pool.tlbr), ptr(self.slots_dev), n, ptr(self.owner), ptr(pool.kp),
+                ptr(pool.kp_count), pool.max_kp, float(self.feat_density), float(self.feat_dist_factor),
+                float(mk["qualityLevel"]), int(mk["maxCorners"]), self.block_size, self.gradient_size,
+                int(self.use_harris), self.harris_k, ptr(self.jobs), ptr(self.scratch), self.scratch_cap,
+                C.c_void_p(fl), C.c_void_p(fl + 4), s), "fm_flow_keypoints_cfg")
         bw, bh = self.bg_feat_sz
         _lib.check(lib.fm_bg_small(ptr(self.gray[self.prev]), ptr(self.owner), W, H, ptr(self.bg), ptr(self.bg_mask),
                                    bw, bh, s), "fm_bg_small")

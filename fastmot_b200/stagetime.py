@@ -15,7 +15,9 @@ STAGE_OF = {
     "fm_yolo_decode_filter": "decode+nms", "fm_diou_nms_filter": "decode+nms",
     "fm_roi_resize_norm": "crops",
     "fm_gray_half": "klt-image", "fm_pyr_level": "klt-image", "fm_scharr": "klt-image", "fm_bg_small": "klt-image",
+    "fm_gray_resize": "klt-image",
     "fm_flow_keypoints": "keypoints", "fm_fast_detect": "keypoints", "fm_gather_points": "keypoints",
+    "fm_flow_keypoints_cfg": "keypoints",
     "fm_lk_track": "lk",
     "fm_ransac_homography": "ransac", "fm_ransac_affine_partial_batch": "ransac",
     "fm_kalman_step_batched": "kalman", "fm_kalman_create_batched": "kalman",

@@ -102,9 +102,10 @@ class MultiTracker:
         self.hist_tracks = OrderedDict()
         self._last_id = 0           # track ids are per tracker: several trackers in one process never share them
         self.kf = KalmanFilter(**vars(kalman_filter_cfg))
-        self.pool = TrackPool(pool_capacity, feat_dim)
         from .flow import Flow
         self.flow = Flow(self.size, **vars(flow_cfg))
+        # keypoint rows sized by obj_feat_params.maxCorners (1024 for the default 1000)
+        self.pool = TrackPool(pool_capacity, feat_dim, max_kp=self.flow.max_kp)
         self.flow.bind_pool(self.pool)
         self.frame_rect = np.array([0., 0., size[0] - 1., size[1] - 1.])
 

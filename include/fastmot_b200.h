@@ -342,6 +342,10 @@ typedef struct FmTrackJob {      /* per-track record produced by fm_flow_keypoin
 
 /* cv2.cvtColor(BGR2GRAY) + cv2.resize(0.5x) of flow.py:153-154 / :129-131 in one pass (w, h even). */
 int fm_gray_half(const unsigned char* frame, int w, int h, unsigned char* gray, unsigned char* small, void* stream);
+/* cv2.cvtColor(BGR2GRAY) + cv2.resize(gray, (sw, sh)) INTER_LINEAR at any optical-flow size 0 < sw <= w,
+ * 0 < sh <= h (odd frame sizes, anisotropic scales, scale 1). */
+int fm_gray_resize(const unsigned char* frame, int w, int h, unsigned char* gray, unsigned char* small, int sw, int sh,
+                   void* stream);
 /* one pyrDown step ((sw+1)/2 x (sh+1)/2) and the Scharr derivative image of a level — what
  * cv2.calcOpticalFlowPyrLK builds internally (flow.py:203-207). */
 int fm_pyr_level(const unsigned char* src, int sw, int sh, unsigned char* dst, void* stream);
@@ -351,13 +355,24 @@ int fm_bg_small(const unsigned char* gray, const int* owner, int w, int h, unsig
                 int bw, int bh, void* stream);
 
 /* flow.py:156-184 for all active tracks (slots[] in nearest-first order, boxes from tlbr_pool): occlusion/owner
- * map, keypoint filtering (_rect_filter), Shi-Tomasi re-detection (cv2.goodFeaturesToTrack, blockSize 3) where
- * len(kp) < feat_density * area, ellipse filter.  Keypoints live in kp_pool[cap][max_kp][2] / kp_count[cap].
- * scratch: scratch_cap floats for the eigenvalue maps; status[0] != 0 reports scratch/candidate overflow. */
+ * map, keypoint filtering (_rect_filter), Shi-Tomasi re-detection (cv2.goodFeaturesToTrack, blockSize 3, gradient
+ * aperture 3, 0 < max_corners <= 1024) where len(kp) < feat_density * area, ellipse filter.  Keypoints live in
+ * kp_pool[cap][max_kp][2] / kp_count[cap].  scratch: scratch_cap floats for the eigenvalue maps; status[0] != 0
+ * reports scratch (2) or candidate (3, more than 4096 local maxima in one box) overflow. */
 int fm_flow_keypoints(const unsigned char* prev_gray, int w, int h, const double* tlbr_pool, const int* slots,
                       int n_trk, int* owner, float* kp_pool, int* kp_count, int max_kp, double feat_density,
                       double feat_dist_factor, double quality, int max_corners, FmTrackJob* jobs, float* scratch,
                       int scratch_cap, int* scratch_counter, int* status, void* stream);
+/* The same for every cv2.goodFeaturesToTrack setting: block_size >= 1 (unnormalised box window anchored at
+ * block_size / 2), gradient_size (Sobel aperture) 1 / 3 / 5 / 7, the minimum-eigenvalue response or, with use_harris,
+ * a*c - b^2 - harris_k*(a+c)^2; max_corners <= 0 keeps every corner.  max_kp must hold min(max_corners, 4096) corners
+ * (4096 when max_corners <= 0).  The default setting runs fm_flow_keypoints; the others use four scratch floats per
+ * crop pixel. */
+int fm_flow_keypoints_cfg(const unsigned char* prev_gray, int w, int h, const double* tlbr_pool, const int* slots,
+                          int n_trk, int* owner, float* kp_pool, int* kp_count, int max_kp, double feat_density,
+                          double feat_dist_factor, double quality, int max_corners, int block_size, int gradient_size,
+                          int use_harris, double harris_k, FmTrackJob* jobs, float* scratch, int scratch_cap,
+                          int* scratch_counter, int* status, void* stream);
 
 /* cv2.FastFeatureDetector(threshold, nonmaxSuppression=True, TYPE_9_16).detect(img, mask) (flow.py:190) followed
  * by _unscale_pts (flow.py:335-344); output points in row-major order. score: w*h scratch bytes. */
@@ -401,8 +416,9 @@ int fm_ransac_affine_partial_batch(const float* all_prev, const float* all_cur, 
 /* ---- KLT stage runner: Flow.predict (flow.py:135-264) as ONE call -------------------------------------------
  * fm_flow_plan_create copies the plan (all pointers are caller-owned device buffers that stay fixed between frames;
  * the fields are the arguments of the per-call functions above, named alike) and creates two private events;
- * fm_flow_predict enqueues, on s_main: gray + 0.5x + pyramid + Scharr of `frame` into buffer 1 - prev, klt_ok clear,
- * fm_flow_keypoints / fm_bg_small / fm_fast_detect / fm_gather_points on buffer prev, fm_lk_track prev -> cur, then
+ * fm_flow_predict enqueues, on s_main: gray + optical-flow image (fm_gray_half when pyr[k].w[0] x h[0] is exactly half
+ * the frame, fm_gray_resize otherwise) + pyramid + Scharr of `frame` into buffer 1 - prev, klt_ok clear,
+ * fm_flow_keypoints_cfg / fm_bg_small / fm_fast_detect / fm_gather_points on buffer prev, fm_lk_track prev -> cur, then
  * fm_ransac_homography on s_side (forked / joined with the private events) next to rounds_ahead (a multiple of 4)
  * rounds of fm_ransac_affine_partial_batch on s_main.  Identical launches to the per-call sequence; no allocation,
  * no synchronisation.  flags: int[32] = {scratch counter, keypoint status, -, .., [8..23] round flags}. */
@@ -456,6 +472,9 @@ typedef struct FmFlowPlan {
     long long klt_ok_bytes;
     double* inlier_ratio;
     int rounds_ahead;
+    /* goodFeaturesToTrack settings of fm_flow_keypoints_cfg (the default: 3, 3, 0, any k) */
+    int block_size, gradient_size, use_harris;
+    double harris_k;
 } FmFlowPlan;
 void* fm_flow_plan_create(const FmFlowPlan* plan);      /* NULL on error (fm_last_error) */
 void fm_flow_plan_destroy(void* handle);
