@@ -14,6 +14,7 @@ import torch
 
 from . import _lib, models
 from .devmem import ptr, stream_ptr, FrameUploader
+from .models.yolo import check_heads
 
 DET_DTYPE = np.dtype(
     [('tlbr', float, 4),
@@ -79,6 +80,7 @@ class YOLODetector(Detector):
         super().__init__(size)
         self._lib = _lib.require_device()
         self.model = models.YOLO.get_model(model)
+        check_heads(self.model)
         assert 0 <= conf_thresh <= 1
         self.conf_thresh = conf_thresh
         assert 0 <= nms_thresh <= 1
@@ -151,6 +153,8 @@ class YOLODetector(Detector):
             engine = build_yolo_engine(self.model, batch=B)
         if getattr(engine, 'batch', 1) != B:
             raise ValueError(f"the engine runs {getattr(engine, 'batch', 1)} images per forward, the detector {B}")
+        if getattr(engine, 'head_shapes', None) is not None:
+            check_heads(self.model, engine.head_shapes)
         self.backend = engine
         self._engines = {B: engine}     # batch k -> engine; k < B share the batch-B engine's resources
 

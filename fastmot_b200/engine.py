@@ -14,6 +14,7 @@ import torch
 from . import _lib
 from .devmem import ptr, stream_ptr
 from .models import darknet, osnet
+from .models.yolo import check_heads
 
 _ACT = darknet.ACTS
 ACT_AFTER_RESIDUAL = 0x100
@@ -197,6 +198,8 @@ class YoloEngine(_Net):
             return t[:B] if B > 1 else t[0]
 
         self.layers, self.shapes = darknet.infer_shapes(layers, 3, H, W)
+        # (c, h, w) of each head per image, in the order forward() returns them
+        self.head_shapes = [self.shapes[i] for i, l in enumerate(self.layers) if l['type'] == 'yolo']
         self.inp = alloc((H, W, IN_C_PAD))
         self.flops = darknet.count_flops(layers, 3, H, W) * B
         L = self.layers
@@ -365,6 +368,7 @@ def build_yolo_engine(model, weights=None, use_tc=True, use_graph=True, head_obj
                                              anchors_per_head=len(model.ANCHORS[0]) // 2)
     else:
         _, layers = darknet.parse_cfg(open(model.CFG).read())
+    check_heads(model, darknet.head_shapes(layers, *model.INPUT_SHAPE[1:]))
     if weights is None:
         if model.WEIGHTS_PATH:
             weights = darknet.load_weights(model.WEIGHTS_PATH, layers, 3)

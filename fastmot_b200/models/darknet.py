@@ -7,11 +7,14 @@ supported layer vocabulary is that script's (`convolutional`, `maxpool`, `route`
   * `load_weights(...)`    — Darknet .weights reader in the converter's order (yolo2onnx.py:283-400): 5 x int32
                              header (major, minor, revision, seen[64-bit if major*10+minor >= 2]), then per conv:
                              BN bias, scale, mean, var (or conv bias) followed by the conv weights [out][in][kh][kw]
-  * builders for the model families named by fastmot/models/yolo.py (tiny / csp / p5 / yolov4).  The official cfg
+  * builders for the eleven models named by fastmot/models/yolo.py (YOLOv3 / -SPP / -tiny, YOLOv4 / -tiny, and the
+    Scaled-YOLOv4 csp / csp-swish / csp-x-swish / x-mish / p5 / p6).  The official cfg
     files are not in the reference tree (downloaded by scripts/download_models.sh), so the builders restate the
     published architectures; `count_flops` reports the Darknet "BFLOPs" figure for a sanity check.
   * `synthetic_weights(...)` — seeded He-normal weights with folded BN (there are no trained weights offline).
 """
+import functools
+
 import numpy as np
 
 ACTS = {'linear': 0, 'leaky': 1, 'mish': 2, 'swish': 3, 'logistic': 4, 'relu': 5}
@@ -159,39 +162,125 @@ def _csp_spp(b, c, act, n=1):
     return b.conv(c, 1, 1, act)
 
 
-def _scaled_yolov4(depths, widths, neck_n, num_classes, anchors_per_head, act='mish'):
+def _scaled_yolov4(depths, widths, neck_n, num_classes, anchors_per_head, act='mish', levels=3, stem=32):
+    """Scaled-YOLOv4 (Wang, Bochkovskiy, Liao, CVPR 2021; models/yolov4-*.yaml of WongKinYiu/ScaledYOLOv4): a stem
+    conv, one CSP stage per entry of widths / depths (each halves the resolution), an SPP-CSP block on the last stage
+    and a PAN neck over the last `levels` stages (level l has width widths[l] / 2, heads twice that).  Heads run finest
+    first (strides 8, 16, ...)."""
     b = _B()
     out_c = anchors_per_head * (5 + num_classes)
-    b.conv(32, 3, 1, act)
+    b.conv(stem, 3, 1, act)
     stage_out = []
     for i, (c, n) in enumerate(zip(widths, depths)):
         stage_out.append(_csp_stage(b, c, n, act, first=(i == 0)))
-    c5 = widths[-1] // 2
-    p5 = _csp_spp(b, c5, act, neck_n)
-    # top-down
-    b.conv(c5 // 2, 1, 1, act); b.upsample()
-    b.route([stage_out[-2]]); b.conv(c5 // 2, 1, 1, act); b.route([-1, -3])
-    p4 = _csp_up(b, c5 // 2, neck_n, act)
-    b.conv(c5 // 4, 1, 1, act); b.upsample()
-    b.route([stage_out[-3]]); b.conv(c5 // 4, 1, 1, act); b.route([-1, -3])
-    p3 = _csp_up(b, c5 // 4, neck_n, act)
-    # heads + bottom-up
-    b.conv(c5 // 2, 3, 1, act); b.conv(out_c, 1, 1, 'logistic', bn=0); b.yolo()
-    b.route([p3]); b.conv(c5 // 2, 3, 2, act); b.route([-1, p4])
-    n4 = _csp_up(b, c5 // 2, neck_n, act)
-    b.conv(c5, 3, 1, act); b.conv(out_c, 1, 1, 'logistic', bn=0); b.yolo()
-    b.route([n4]); b.conv(c5, 3, 2, act); b.route([-1, p5])
-    _csp_up(b, c5, neck_n, act)
-    b.conv(c5 * 2, 3, 1, act); b.conv(out_c, 1, 1, 'logistic', bn=0); b.yolo()
+    stage_out = stage_out[-levels:]
+    nw = [c // 2 for c in widths[-levels:]]
+    td = [None] * (levels - 1) + [_csp_spp(b, nw[-1], act, neck_n)]
+    for l in range(levels - 2, -1, -1):           # top-down
+        b.conv(nw[l], 1, 1, act); b.upsample()
+        b.route([stage_out[l]]); b.conv(nw[l], 1, 1, act); b.route([-1, -3])
+        td[l] = _csp_up(b, nw[l], neck_n, act)
+    prev = td[0]
+    for l in range(levels):                       # heads + bottom-up
+        if l:
+            b.route([prev]); b.conv(nw[l], 3, 2, act); b.route([-1, td[l]])
+            prev = _csp_up(b, nw[l], neck_n, act)
+        b.conv(2 * nw[l], 3, 1, act); b.conv(out_c, 1, 1, 'logistic', bn=0); b.yolo()
     return b.layers
 
 
-def yolov4_csp(num_classes=1, anchors_per_head=3):
-    return _scaled_yolov4([1, 2, 8, 8, 4], [64, 128, 256, 512, 1024], 2, num_classes, anchors_per_head)
+def yolov4_csp(num_classes=1, anchors_per_head=3, act='mish'):
+    """YOLOv4-CSP (ScaledYOLOv4 models/yolov4-csp.yaml; Darknet yolov4-csp.cfg, and yolov4-csp-swish.cfg with
+    act='swish')."""
+    return _scaled_yolov4([1, 2, 8, 8, 4], [64, 128, 256, 512, 1024], 2, num_classes, anchors_per_head, act)
 
 
 def yolov4_p5(num_classes=1, anchors_per_head=4):
     return _scaled_yolov4([1, 3, 15, 15, 7], [64, 128, 256, 512, 1024], 3, num_classes, anchors_per_head)
+
+
+def yolov4_csp_x(num_classes=1, anchors_per_head=3, act='mish'):
+    """YOLOv4-CSP-x: yolov4-csp at width multiple 1.25 and depth multiple 1.33 (ScaledYOLOv4 models/yolov4-csp-x.yaml;
+    the Darknet yolov4x-mish.cfg / yolov4-csp-x-swish.cfg): stem 40, stages 80 ... 1280 with depths 1 / 3 / 11 / 11 / 5,
+    neck depth 3."""
+    return _scaled_yolov4([1, 3, 11, 11, 5], [80, 160, 320, 640, 1280], 3, num_classes, anchors_per_head, act,
+                          stem=40)
+
+
+def yolov4_p6(num_classes=1, anchors_per_head=4):
+    """YOLOv4-P6 (ScaledYOLOv4 models/yolov4-p6.yaml, Darknet yolov4-p6.cfg): the P5 backbone plus a sixth stage
+    (1024 wide, 7 units) at stride 64, the SPP-CSP block on it and a four-level neck (widths 128 / 256 / 512 / 512),
+    four heads at strides 8 / 16 / 32 / 64."""
+    return _scaled_yolov4([1, 3, 15, 15, 7, 7], [64, 128, 256, 512, 1024, 1024], 3, num_classes, anchors_per_head,
+                          levels=4)
+
+
+def _darknet53(b):
+    """Darknet-53 (Redmon & Farhadi, "YOLOv3: An Incremental Improvement", 2018; cfg/yolov3.cfg layers 0-74): returns
+    the layer indices of its five stage outputs (strides 2 ... 32)."""
+    b.conv(32, 3, 1)
+    outs = []
+    for c, n in zip((64, 128, 256, 512, 1024), (1, 2, 8, 8, 4)):
+        b.conv(c, 3, 2)
+        for _ in range(n):
+            b.conv(c // 2, 1, 1); b.conv(c, 3, 1); b.shortcut(-3)
+        outs.append(len(b.layers) - 1)
+    return outs
+
+
+def _yolov3(num_classes, anchors_per_head, spp):
+    b = _B()
+    out_c = anchors_per_head * (5 + num_classes)
+    outs = _darknet53(b)
+    x = None
+    for lvl, c in enumerate((512, 256, 128)):     # heads coarsest first (strides 32, 16, 8)
+        if lvl:
+            b.route([x]); b.conv(c, 1, 1); b.upsample(); b.route([-1, outs[4 - lvl]])
+        b.conv(c, 1, 1); b.conv(2 * c, 3, 1); b.conv(c, 1, 1)
+        if spp and not lvl:
+            b.maxpool(5, 1); b.route([-2]); b.maxpool(9, 1); b.route([-4]); b.maxpool(13, 1)
+            b.route([-1, -3, -5, -6])
+            b.conv(c, 1, 1)
+        b.conv(2 * c, 3, 1)
+        x = b.conv(c, 1, 1)
+        b.conv(2 * c, 3, 1)
+        b.conv(out_c, 1, 1, 'linear', bn=0)
+        b.yolo()
+    return b.layers
+
+
+def yolov3(num_classes=1, anchors_per_head=3):
+    """YOLOv3 (cfg/yolov3.cfg of pjreddie/darknet): Darknet-53 + an FPN of three heads, 107 layers."""
+    return _yolov3(num_classes, anchors_per_head, spp=False)
+
+
+def yolov3_spp(num_classes=1, anchors_per_head=3):
+    """YOLOv3-SPP (cfg/yolov3-spp.cfg of pjreddie/darknet): YOLOv3 with a 5 / 9 / 13 max-pool SPP block in the
+    stride-32 head, 114 layers."""
+    return _yolov3(num_classes, anchors_per_head, spp=True)
+
+
+def yolov3_tiny(num_classes=1, anchors_per_head=3):
+    """YOLOv3-tiny (cfg/yolov3-tiny.cfg of pjreddie/darknet): six 3x3 convs each followed by a 2x2 max-pool (the last
+    one at stride 1), two heads (strides 32, 16), 24 layers."""
+    b = _B()
+    out_c = anchors_per_head * (5 + num_classes)
+    for c in (16, 32, 64, 128, 256, 512):
+        b.conv(c, 3, 1)
+        b.maxpool(2, 1 if c == 512 else 2)
+    b.conv(1024, 3, 1)
+    p = b.conv(256, 1, 1)
+    b.conv(512, 3, 1)
+    b.conv(out_c, 1, 1, 'linear', bn=0)
+    b.yolo()
+    b.route([p])
+    b.conv(128, 1, 1)
+    b.upsample()
+    b.route([-1, 8])                              # the 256-wide conv at stride 16
+    b.conv(256, 3, 1)
+    b.conv(out_c, 1, 1, 'linear', bn=0)
+    b.yolo()
+    return b.layers
 
 
 def yolov4(num_classes=2, anchors_per_head=3):
@@ -234,7 +323,16 @@ def yolov4(num_classes=2, anchors_per_head=3):
     return b.layers
 
 
-BUILDERS = {'yolov4-tiny': yolov4_tiny, 'yolov4-csp': yolov4_csp, 'yolov4-p5': yolov4_p5, 'yolov4': yolov4}
+BUILDERS = {'yolov4-tiny': yolov4_tiny, 'yolov4-csp': yolov4_csp, 'yolov4-p5': yolov4_p5, 'yolov4': yolov4,
+            'yolov3': yolov3, 'yolov3-spp': yolov3_spp, 'yolov3-tiny': yolov3_tiny,
+            'yolov4x-mish': yolov4_csp_x, 'yolov4-csp-swish': functools.partial(yolov4_csp, act='swish'),
+            'yolov4-csp-x-swish': functools.partial(yolov4_csp_x, act='swish'), 'yolov4-p6': yolov4_p6}
+
+
+def head_shapes(layers, in_h, in_w):
+    """(c, h, w) of every [yolo] layer's input, in graph order, for an in_h x in_w network input."""
+    res, shapes = infer_shapes(layers, 3, in_h, in_w)
+    return [shapes[i] for i, l in enumerate(res) if l['type'] == 'yolo']
 
 
 # ------------------------------------------------------------------------------------------------ shape inference
@@ -308,7 +406,10 @@ def synthetic_weights(layers, in_c, seed_base=1000, head_obj_bias=None, num_clas
         out[i] = (w, b)
     if calibrate:
         from .calibrate import calibrate_darknet
-        out = calibrate_darknet(res, out, in_c)
+        # a 4 x 4 grid at the coarsest stride at least: the channel statistics of P6's stride-64 stage taken on 2 x 2
+        # pixels leave its activations past the fp16 range at 1280 (strides up to 32 calibrate at 128, as before)
+        stride = 64 // min(s[1] for s in infer_shapes(layers, in_c, 64, 64)[1])
+        out = calibrate_darknet(res, out, in_c, size=max(128, 4 * stride))
     if head_gain != 1.0:
         for i, l in enumerate(res):
             if l['type'] == 'convolutional' and i + 1 < len(res) and res[i + 1]['type'] == 'yolo':
