@@ -105,7 +105,9 @@ __global__ void __launch_bounds__(256) matching_cost_kernel(
                 c = (1.0 - motion_weight) * c + motion_weight * (1.0 / FM_CHI_SQ_INV_95) * m;
                 if (m > FM_CHI_SQ_INV_95) c = FM_INF_COST;
             }
-            if ((det_labels && tl != det_labels[dj]) || (max_cost >= 0.0 && c > max_cost)) c = FM_INF_COST;
+            // label gate only when both sides have labels, as in iou_cost_kernel
+            if ((trk_labels && det_labels && tl != det_labels[dj]) || (max_cost >= 0.0 && c > max_cost))
+                c = FM_INF_COST;
             cost[(size_t)i * n_det + j] = c;
         }
     }

@@ -89,6 +89,7 @@ int fm_motion_distance(const double* mean_pool, const double* cov_pool, const in
  * feat_pool[cap][dim] f32 running-average features, feat_valid_pool[cap] (count > 0);
  * trk_slots[n_trk], trk_labels[n_trk]; det_* arrays have n_det rows, det_sel[n_det] (NULL = identity) selects
  * the rows of the full detection arrays that are still unmatched.  cost[n_trk][n_det] f64 row-major.
+ * The label gate applies only when both trk_labels and det_labels are non-NULL (as in fm_iou_cost).
  * motion_weight < 0 disables the motion term; max_cost < 0 disables the cost gate (tracker.py:355-366 re-ID). */
 int fm_matching_cost(const float* feat_pool, const unsigned char* feat_valid_pool, const double* mean_pool,
                      const double* cov_pool, const int* trk_slots, const long long* trk_labels, int n_trk,
@@ -104,7 +105,8 @@ int fm_feature_update(float* sum_pool, float* avg_pool, float* last_pool, unsign
                       const float* vec, const int* vec_idx, const int* counts, int n, int dim, void* stream);
 
 /* iou_dist (distance.py:90-108) + gate_cost (matching.py:109-116); boxes gathered by index lists.
- * trk_tlbr_pool[cap][4]; labels may be NULL (no label gate), max_cost < 0 disables the cost gate. */
+ * trk_tlbr_pool[cap][4]; the label gate applies only when both label arrays are non-NULL, max_cost < 0 disables the
+ * cost gate. */
 int fm_iou_cost(const double* trk_tlbr_pool, const int* trk_slots, const long long* trk_labels, int n_trk,
                 const double* det_tlbr, const long long* det_labels, const int* det_sel, int n_det,
                 double max_cost, double* cost, void* stream);
