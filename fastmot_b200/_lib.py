@@ -108,14 +108,10 @@ SIGNATURES = {
     "fm_assoc_cascade_out_ints": (c_ll, [c_i]),
     "fm_letterbox_preproc": (c_i, [c_p, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_p, c_p]),
     "fm_roi_resize_norm": (c_i, [c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p]),
-    "fm_letterbox_preproc_batch": (c_i, [c_p, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_p, c_p]),
-    "fm_roi_resize_norm_multi": (c_i, [c_p, c_p, c_i, c_i, c_p, c_i, c_i, c_i, c_i, c_p, c_p]),
     "fm_letterbox_preproc_geom": (c_i, [c_p, c_i, c_i, c_i, c_p, c_p]),
     "fm_roi_resize_norm_geom": (c_i, [c_p, c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p]),
     "fm_yolo_decode_filter_geom": (c_i, [c_p, c_i, c_ll, c_i, c_i, c_i, c_i, c_i, C.POINTER(FmYoloHead), c_i, c_i,
                                           c_i, c_i, c_i, c_i, c_p, c_d, c_p, c_p, c_p, c_p, c_i, c_p]),
-    "fm_yolo_decode_filter_batch": (c_i, [c_p, c_i, c_ll, c_i, c_i, c_i, c_i, c_i, C.POINTER(FmYoloHead), c_i, c_i,
-                                           c_i, c_i, c_i, c_i, c_p, c_d, c_f, c_f, c_f, c_f, c_p, c_p, c_p, c_i, c_p]),
     "fm_diou_nms_filter_batch": (c_i, [c_i, c_p, c_p, c_i, c_p, c_i, c_d, c_d, c_d, c_p, c_i, c_p, c_p, c_p, c_p, c_p,
                                         c_p]),
     "fm_yolo_decode_filter": (c_i, [c_p, c_i, c_i, c_i, c_i, c_i, C.POINTER(FmYoloHead), c_i, c_i, c_i, c_i, c_i, c_p,

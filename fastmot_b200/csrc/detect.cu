@@ -11,8 +11,8 @@
 // dense rows + b * cand_stride, keys + b * key_cap, counter[b], mask + b * key_cap * words, outputs + b * max_out,
 // out_count[b], status[b]) and the grid carries b.  The one-image entries launch the same kernels with one image, so
 // a batched image's keys, rows and detections are those of the one-image path on the same head slice, and NMS never
-// compares boxes of different images.  The *_geom entry reads each image's pixel scale and letterbox offset from a
-// device FmFrameGeom table instead of taking one for the whole batch (images of different frame sizes).
+// compares boxes of different images.  The batched decode (fm_yolo_decode_filter_geom) reads each image's pixel scale
+// and letterbox offset from a device FmFrameGeom table, so the images of one batch may come from frames of any sizes.
 #include "common.cuh"
 #include "../../include/fastmot_b200.h"
 
@@ -203,52 +203,6 @@ __global__ void __launch_bounds__(64) nms_mask_kernel(const unsigned long long* 
     }
 }
 
-// Serial greedy scan (one warp) + final filters + ordered output (detector.py:357-365).
-__global__ void __launch_bounds__(32) nms_scan_kernel(const unsigned long long* __restrict__ keys,
-                                                       const float* __restrict__ dense,
-                                                       const int* __restrict__ counter, int key_cap,
-                                                       const unsigned long long* __restrict__ mask, int mask_words,
-                                                       double max_area, double min_ar, int max_out,
-                                                       double* __restrict__ out_tlbr, long long* __restrict__ out_label,
-                                                       double* __restrict__ out_conf, int* __restrict__ out_count) {
-    extern __shared__ unsigned long long removed[];
-    const int lane = threadIdx.x;
-    int n = min(*counter, key_cap);
-    const int nw = (n + 63) >> 6;
-    for (int w = lane; w < nw; w += 32) removed[w] = 0;
-    __syncwarp();
-    int nout = 0;
-    for (int i = 0; i < n; ++i) {
-        const bool dead = (removed[i >> 6] >> (i & 63)) & 1ull;
-        if (dead) continue;  // warp-uniform (shared state)
-        for (int w = (i >> 6) + lane; w < nw; w += 32) removed[w] |= mask[(size_t)i * mask_words + w];
-        __syncwarp();
-        if (lane == 0) {
-            const float* d = dense + (size_t)(keys[i] & 0xffffff) * 8;
-            const double xmin = (double)d[0], ymin = (double)d[1];
-            const double x1 = rint(xmin), y1 = rint(ymin);
-            // to_tlbr under Numba: x + w is an f32 add, the `- 1.` literal promotes to f64 (oracle/detect.py)
-            const double x2 = rint((double)(d[0] + d[2]) - 1.0), y2 = rint((double)(d[1] + d[3]) - 1.0);
-            const double w = x2 - x1 + 1.0, h = y2 - y1 + 1.0;
-            const double area = (w <= 0 || h <= 0) ? 0.0 : w * h;
-            const double ar = w > 0 ? h / w : 0.0;
-            if (area > 0 && area <= max_area && ar >= min_ar && nout < max_out) {
-                out_tlbr[nout * 4 + 0] = x1; out_tlbr[nout * 4 + 1] = y1;
-                out_tlbr[nout * 4 + 2] = x2; out_tlbr[nout * 4 + 3] = y2;
-                out_label[nout] = (long long)d[5];
-                out_conf[nout] = (double)__fmul_rn(d[4], d[6]);
-                removed[nw] = 1;  // scratch flag: accepted
-            } else {
-                removed[nw] = 0;
-            }
-        }
-        __syncwarp();
-        nout += (int)removed[nw];
-        __syncwarp();
-    }
-    if (lane == 0) *out_count = nout;
-}
-
 }  // namespace
 
 static int launch_decode(const void* head_out, int batch, long long head_stride, int cand_stride, int is_fp16, int nhwc,
@@ -285,24 +239,6 @@ extern "C" int fm_yolo_decode_filter(const void* head_out, int is_fp16, int nhwc
     return launch_decode(head_out, 1, 0, 0, is_fp16, nhwc, yolo_w, yolo_h, num_anchors, *head, num_classes, input_w,
                          input_h, new_coords, cand_base, label_mask, conf_thresh, size_w, size_h, off_x, off_y, nullptr,
                          dense, keys, counter, key_cap, stream, "fm_yolo_decode_filter");
-}
-
-extern "C" int fm_yolo_decode_filter_batch(const void* head_out, int batch, long long head_stride, int is_fp16,
-                                           int nhwc, int yolo_w, int yolo_h, int num_anchors, const FmYoloHead* head,
-                                           int num_classes, int input_w, int input_h, int new_coords, int cand_base,
-                                           int cand_stride, const unsigned char* label_mask, double conf_thresh,
-                                           float size_w, float size_h, float off_x, float off_y, float* dense,
-                                           unsigned long long* keys, int* counters, int key_cap, void* stream) {
-    FM_REQUIRE(head != nullptr, "fm_yolo_decode_filter_batch: head is NULL");
-    FM_REQUIRE(num_anchors <= FM_MAX_ANCHORS, "fm_yolo_decode_filter_batch: too many anchors");
-    FM_REQUIRE(batch > 0 && batch <= 65535, "fm_yolo_decode_filter_batch: batch must be in [1, 65535]");
-    FM_REQUIRE(cand_base + yolo_w * yolo_h * num_anchors <= cand_stride && cand_stride <= (1 << 24),
-               "fm_yolo_decode_filter_batch: the head's candidates do not fit in cand_stride (<= 2^24) rows per image");
-    FM_REQUIRE(head_stride >= (long long)yolo_w * yolo_h * num_anchors * (5 + num_classes),
-               "fm_yolo_decode_filter_batch: head_stride is smaller than one image's head");
-    return launch_decode(head_out, batch, head_stride, cand_stride, is_fp16, nhwc, yolo_w, yolo_h, num_anchors, *head,
-                         num_classes, input_w, input_h, new_coords, cand_base, label_mask, conf_thresh, size_w, size_h,
-                         off_x, off_y, nullptr, dense, keys, counters, key_cap, stream, "fm_yolo_decode_filter_batch");
 }
 
 extern "C" int fm_yolo_decode_filter_geom(const void* head_out, int batch, long long head_stride, int is_fp16,
@@ -350,7 +286,7 @@ static int launch_nms(int batch, unsigned long long* keys, const float* dense, i
     FM_CHECK_LAUNCH("nms_mask_kernel");
     fm_launch_nms_scan(batch, keys, dense, cand_stride, counter, key_cap, mask, words, max_area, min_aspect_ratio,
                        max_out, out_tlbr, out_label, out_conf, out_count, status, s);   // blocked scan, detect_nms.cu
-    FM_CHECK_LAUNCH("nms_scan_kernel");
+    FM_CHECK_LAUNCH("nms_scan_blocked_kernel");
     return FM_OK;
 }
 

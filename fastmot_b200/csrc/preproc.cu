@@ -4,10 +4,9 @@
 //   fm_roi_resize_norm   : per-detection crop + OpenCV-style fixed-point bilinear resize to 128x256 + ImageNet
 //                          normalisation, all crops in one launch (fastmot/feature_extractor.py:48-60, 84-98;
 //                          fastmot/utils/rect.py:92-97)
-// The *_batch / *_multi entries run the same kernels over a device table of frame pointers (one grid slice per
-// frame, or one frame index per crop), so every pixel is computed by the same code as in the one-frame entries.
-// The *_geom entries read each frame's pointer, size (and, for the letterbox, ROI) from a device FmFrameGeom table,
-// so one launch covers frames of different sizes; again the kernel body is the one-frame entries'.
+// The *_geom entries read each frame's pointer, size (and, for the letterbox, ROI) from a device FmFrameGeom table
+// (one grid slice per frame, or one frame index per crop), so one launch covers several frames of any sizes; every
+// pixel is computed by the same kernel body as in the one-frame entries.
 // Outputs are either fp32 planar CHW (the reference's TensorRT input layout; used for parity tests) or fp16
 // NHWC with C padded to 8 (one 16-byte chunk per pixel; what the conv engine consumes).
 #include "common.cuh"
@@ -39,11 +38,10 @@ __device__ __forceinline__ void store_px(void* out, int H, int W, int y, int x, 
     }
 }
 
-// frames != nullptr: image blockIdx.z reads frames[blockIdx.z] and writes the blockIdx.z-th NHWC8 image of out;
-// geom != nullptr: likewise, with the frame, its size and its ROI taken from geom[blockIdx.z]
+// geom != nullptr: image blockIdx.z takes its frame, size and ROI from geom[blockIdx.z] and writes the blockIdx.z-th
+// NHWC8 image of out
 template <int LAYOUT>
 __global__ void __launch_bounds__(256) letterbox_kernel(const unsigned char* __restrict__ frame,
-                                                         const unsigned char* const* __restrict__ frames,
                                                          const FmFrameGeom* __restrict__ geom, int src_w,
                                                          int src_h, int dst_w, int dst_h, int roi_x, int roi_y,
                                                          int roi_w, int roi_h, void* __restrict__ out) {
@@ -55,9 +53,6 @@ __global__ void __launch_bounds__(256) letterbox_kernel(const unsigned char* __r
         frame = g.frame;
         src_w = g.w; src_h = g.h;
         roi_x = g.roi_x; roi_y = g.roi_y; roi_w = g.roi_w; roi_h = g.roi_h;
-        out = (__half*)out + (size_t)blockIdx.z * dst_h * dst_w * 8;
-    } else if (frames != nullptr) {
-        frame = frames[blockIdx.z];
         out = (__half*)out + (size_t)blockIdx.z * dst_h * dst_w * 8;
     }
     const int rx = x - roi_x, ry = y - roi_y;
@@ -101,11 +96,9 @@ __device__ __forceinline__ void cv_coef(int d, double scale, int ssize, int& s, 
     a1 = (int)rintf(f * 2048.f);
 }
 
-// frames != nullptr: crop i is cut from frames[frame_idx[i]]; geom != nullptr: from geom[frame_idx[i]].frame, with
-// that frame's own width and height
+// geom != nullptr: crop i is cut from geom[frame_idx[i]].frame, with that frame's own width and height
 template <int LAYOUT>
 __global__ void __launch_bounds__(128) roi_resize_norm_kernel(const unsigned char* __restrict__ frame,
-                                                               const unsigned char* const* __restrict__ frames,
                                                                const FmFrameGeom* __restrict__ geom,
                                                                const int* __restrict__ frame_idx, int src_w,
                                                                int src_h, const double* __restrict__ tlbrs,
@@ -118,8 +111,6 @@ __global__ void __launch_bounds__(128) roi_resize_norm_kernel(const unsigned cha
         const FmFrameGeom& g = geom[frame_idx[crop]];
         frame = g.frame;
         src_w = g.w; src_h = g.h;
-    } else if (frames != nullptr) {
-        frame = frames[frame_idx[crop]];
     }
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y;
@@ -161,10 +152,10 @@ extern "C" int fm_letterbox_preproc(const unsigned char* frame, int src_w, int s
     FM_REQUIRE(roi_w > 0 && roi_h > 0, "fm_letterbox_preproc: empty ROI");
     dim3 grid(fm_cdiv(dst_w, 256), dst_h);
     if (layout == 0)
-        letterbox_kernel<0><<<grid, 256, 0, (cudaStream_t)stream>>>(frame, nullptr, nullptr, src_w, src_h, dst_w, dst_h, roi_x, roi_y,
+        letterbox_kernel<0><<<grid, 256, 0, (cudaStream_t)stream>>>(frame, nullptr, src_w, src_h, dst_w, dst_h, roi_x, roi_y,
                                                                     roi_w, roi_h, out);
     else
-        letterbox_kernel<1><<<grid, 256, 0, (cudaStream_t)stream>>>(frame, nullptr, nullptr, src_w, src_h, dst_w, dst_h, roi_x, roi_y,
+        letterbox_kernel<1><<<grid, 256, 0, (cudaStream_t)stream>>>(frame, nullptr, src_w, src_h, dst_w, dst_h, roi_x, roi_y,
                                                                     roi_w, roi_h, out);
     FM_CHECK_LAUNCH("fm_letterbox_preproc");
     return FM_OK;
@@ -178,49 +169,15 @@ extern "C" int fm_roi_resize_norm(const unsigned char* frame, int src_w, int src
     FM_REQUIRE(n_max <= 65535, "fm_roi_resize_norm: more than 65535 crops");
     dim3 grid(fm_cdiv(out_w, 128), out_h, n_max);
     if (layout == 0)
-        roi_resize_norm_kernel<0><<<grid, 128, 0, (cudaStream_t)stream>>>(frame, nullptr, nullptr, nullptr, src_w, src_h, tlbrs, n_dev, n_max,
+        roi_resize_norm_kernel<0><<<grid, 128, 0, (cudaStream_t)stream>>>(frame, nullptr, nullptr, src_w, src_h, tlbrs, n_dev, n_max,
                                                                           out_w, out_h, out);
     else if (layout == 1)
-        roi_resize_norm_kernel<1><<<grid, 128, 0, (cudaStream_t)stream>>>(frame, nullptr, nullptr, nullptr, src_w, src_h, tlbrs, n_dev, n_max,
+        roi_resize_norm_kernel<1><<<grid, 128, 0, (cudaStream_t)stream>>>(frame, nullptr, nullptr, src_w, src_h, tlbrs, n_dev, n_max,
                                                                           out_w, out_h, out);
     else
-        roi_resize_norm_kernel<2><<<grid, 128, 0, (cudaStream_t)stream>>>(frame, nullptr, nullptr, nullptr, src_w, src_h, tlbrs, n_dev, n_max,
+        roi_resize_norm_kernel<2><<<grid, 128, 0, (cudaStream_t)stream>>>(frame, nullptr, nullptr, src_w, src_h, tlbrs, n_dev, n_max,
                                                                           out_w, out_h, out);
     FM_CHECK_LAUNCH("fm_roi_resize_norm");
-    return FM_OK;
-}
-
-extern "C" int fm_letterbox_preproc_batch(const unsigned char* const* frames, int batch, int src_w, int src_h,
-                                          int dst_w, int dst_h, int roi_x, int roi_y, int roi_w, int roi_h, void* out,
-                                          void* stream) {
-    FM_REQUIRE(frames != nullptr, "fm_letterbox_preproc_batch: frame table is NULL");
-    FM_REQUIRE(batch > 0 && batch <= 65535, "fm_letterbox_preproc_batch: batch must be in [1, 65535]");
-    FM_REQUIRE(roi_w > 0 && roi_h > 0, "fm_letterbox_preproc_batch: empty ROI");
-    dim3 grid(fm_cdiv(dst_w, 256), dst_h, batch);
-    letterbox_kernel<1><<<grid, 256, 0, (cudaStream_t)stream>>>(nullptr, frames, nullptr, src_w, src_h, dst_w, dst_h, roi_x,
-                                                                roi_y, roi_w, roi_h, out);
-    FM_CHECK_LAUNCH("fm_letterbox_preproc_batch");
-    return FM_OK;
-}
-
-extern "C" int fm_roi_resize_norm_multi(const unsigned char* const* frames, const int* frame_idx, int src_w,
-                                        int src_h, const double* tlbrs, int n, int out_w, int out_h, int layout,
-                                        void* out, void* stream) {
-    FM_REQUIRE(layout >= 0 && layout <= 2, "fm_roi_resize_norm_multi: layout must be 0 (f32 CHW), 1 (f16 NHWC8) or 2 (f16 NHWC4, padded)");
-    if (n <= 0) return FM_OK;
-    FM_REQUIRE(frames != nullptr && frame_idx != nullptr, "fm_roi_resize_norm_multi: frame table or index is NULL");
-    FM_REQUIRE(n <= 65535, "fm_roi_resize_norm_multi: more than 65535 crops");
-    dim3 grid(fm_cdiv(out_w, 128), out_h, n);
-    if (layout == 0)
-        roi_resize_norm_kernel<0><<<grid, 128, 0, (cudaStream_t)stream>>>(nullptr, frames, nullptr, frame_idx, src_w, src_h,
-                                                                          tlbrs, nullptr, n, out_w, out_h, out);
-    else if (layout == 1)
-        roi_resize_norm_kernel<1><<<grid, 128, 0, (cudaStream_t)stream>>>(nullptr, frames, nullptr, frame_idx, src_w, src_h,
-                                                                          tlbrs, nullptr, n, out_w, out_h, out);
-    else
-        roi_resize_norm_kernel<2><<<grid, 128, 0, (cudaStream_t)stream>>>(nullptr, frames, nullptr, frame_idx, src_w, src_h,
-                                                                          tlbrs, nullptr, n, out_w, out_h, out);
-    FM_CHECK_LAUNCH("fm_roi_resize_norm_multi");
     return FM_OK;
 }
 
@@ -229,7 +186,7 @@ extern "C" int fm_letterbox_preproc_geom(const FmFrameGeom* geom, int batch, int
     FM_REQUIRE(geom != nullptr, "fm_letterbox_preproc_geom: geometry table is NULL");
     FM_REQUIRE(batch > 0 && batch <= 65535, "fm_letterbox_preproc_geom: batch must be in [1, 65535]");
     dim3 grid(fm_cdiv(dst_w, 256), dst_h, batch);
-    letterbox_kernel<1><<<grid, 256, 0, (cudaStream_t)stream>>>(nullptr, nullptr, geom, 0, 0, dst_w, dst_h, 0, 0, 0, 0,
+    letterbox_kernel<1><<<grid, 256, 0, (cudaStream_t)stream>>>(nullptr, geom, 0, 0, dst_w, dst_h, 0, 0, 0, 0,
                                                                 out);
     FM_CHECK_LAUNCH("fm_letterbox_preproc_geom");
     return FM_OK;
@@ -243,13 +200,13 @@ extern "C" int fm_roi_resize_norm_geom(const FmFrameGeom* geom, const int* frame
     FM_REQUIRE(n <= 65535, "fm_roi_resize_norm_geom: more than 65535 crops");
     dim3 grid(fm_cdiv(out_w, 128), out_h, n);
     if (layout == 0)
-        roi_resize_norm_kernel<0><<<grid, 128, 0, (cudaStream_t)stream>>>(nullptr, nullptr, geom, frame_idx, 0, 0,
+        roi_resize_norm_kernel<0><<<grid, 128, 0, (cudaStream_t)stream>>>(nullptr, geom, frame_idx, 0, 0,
                                                                           tlbrs, nullptr, n, out_w, out_h, out);
     else if (layout == 1)
-        roi_resize_norm_kernel<1><<<grid, 128, 0, (cudaStream_t)stream>>>(nullptr, nullptr, geom, frame_idx, 0, 0,
+        roi_resize_norm_kernel<1><<<grid, 128, 0, (cudaStream_t)stream>>>(nullptr, geom, frame_idx, 0, 0,
                                                                           tlbrs, nullptr, n, out_w, out_h, out);
     else
-        roi_resize_norm_kernel<2><<<grid, 128, 0, (cudaStream_t)stream>>>(nullptr, nullptr, geom, frame_idx, 0, 0,
+        roi_resize_norm_kernel<2><<<grid, 128, 0, (cudaStream_t)stream>>>(nullptr, geom, frame_idx, 0, 0,
                                                                           tlbrs, nullptr, n, out_w, out_h, out);
     FM_CHECK_LAUNCH("fm_roi_resize_norm_geom");
     return FM_OK;

@@ -74,9 +74,8 @@ class YOLODetector(Detector):
                  engine=None,
                  batch=1):
         """batch = B > 1: the detector runs up to B frames per forward (detect_batch_async / postprocess_batch);
-        key_cap and max_dets then hold per image.  B frames of `size` run the batch-B engine with this size's
-        geometry; any other set of 1..B frames (any sizes) runs the engine of its own batch k, which shares the batch-B
-        engine's weights and buffers, with each frame's geometry taken from its shape."""
+        key_cap and max_dets then hold per image.  k frames of any sizes run the engine of batch k (at k < B it shares
+        the batch-B engine's weights and buffers), each frame with the letterbox and box geometry of its own size."""
         super().__init__(size)
         self._lib = _lib.require_device()
         self.model = models.YOLO.get_model(model)
@@ -136,10 +135,7 @@ class YOLODetector(Detector):
         self.inp = torch.zeros(lead + (in_h, in_w, 8), dtype=torch.float16, device=dev)   # NHWC8
         self._uploader = FrameUploader(size)
         self._uploaders = [self._uploader] + [None] * (B - 1)    # built on the first host frame of their slot
-        self._frame_tab_h = torch.zeros(B, dtype=torch.int64).pin_memory()     # frame pointers of detect_batch_async
-        self._frame_tab = torch.zeros(B, dtype=torch.int64, device=dev)
-        self._frame_tab_ev = None
-        # per-frame geometry (one FmFrameGeom row per image) of the frames that are not B frames of `size`
+        # per-frame geometry of detect_batch_async (one FmFrameGeom row per image)
         self._geom_bytes = C.sizeof(_lib.FmFrameGeom)
         self._geom_h = torch.zeros(B * self._geom_bytes, dtype=torch.uint8).pin_memory()
         self._geom = torch.zeros(B * self._geom_bytes, dtype=torch.uint8, device=dev)
@@ -209,58 +205,39 @@ class YOLODetector(Detector):
         """Waits for the async pipeline and returns np.recarray[DET_DTYPE] (class asc, objectness desc)."""
         self._done.synchronize()
         n, status, n_cand = (int(v) for v in self._h_meta[:3])
+        dets = self._image_dets(n, status, n_cand, 0)
+        self.last_num_candidates = n_cand
+        return dets
+
+    def _image_dets(self, n, status, n_cand, row0, name=None):
+        """One image's n detections, rows [row0, row0 + n) of the host outputs, as np.recarray[DET_DTYPE].  Its NMS
+        status raises on an overflow; the message starts with `name` when one is given."""
+        prefix = "" if name is None else f"{name}: "
         if status == 2:
-            raise RuntimeError(f"more than max_dets = {self.max_dets} boxes survived NMS and the area / aspect "
+            raise RuntimeError(f"{prefix}more than max_dets = {self.max_dets} boxes survived NMS and the area / aspect "
                                "filters; raise max_dets (no silent truncation)")
         if status != 0:
-            raise RuntimeError(f"{n_cand} candidates passed conf_thresh but key_cap is {self.key_cap}; "
+            raise RuntimeError(f"{prefix}{n_cand} candidates passed conf_thresh but key_cap is {self.key_cap}; "
                                "raise key_cap (no silent truncation)")
-        self.last_num_candidates = n_cand
         dets = np.zeros(n, DET_DTYPE)
-        dets['tlbr'] = self._h_tlbr.numpy()[:n]
-        dets['label'] = self._h_label.numpy()[:n]
-        dets['conf'] = self._h_conf.numpy()[:n]
+        dets['tlbr'] = self._h_tlbr.numpy()[row0:row0 + n]
+        dets['label'] = self._h_label.numpy()[row0:row0 + n]
+        dets['conf'] = self._h_conf.numpy()[row0:row0 + n]
         return dets.view(np.recarray)
 
     # ------------------------------------------------------------------ batch > 1
-    def preprocess_batch(self, frames_dev):
-        """Letterbox of the B frames (HxWx3 u8 cuda tensors of this detector's size) into self.inp, one launch."""
-        B = self.batch
-        if len(frames_dev) != B:
-            raise ValueError(f"expected {B} frames, got {len(frames_dev)}")
-        want = (self.size[1], self.size[0], 3)
-        for f in frames_dev:
-            if tuple(f.shape) != want or f.dtype != torch.uint8 or not f.is_contiguous() or not f.is_cuda:
-                raise ValueError(f"every frame must be a contiguous uint8 cuda tensor of shape {want}")
-        if self._frame_tab_ev is not None:
-            self._frame_tab_ev.synchronize()        # the previous table upload has left the pinned block
-        self._frame_tab_h.copy_(torch.tensor([f.data_ptr() for f in frames_dev], dtype=torch.int64))
-        self._frame_tab.copy_(self._frame_tab_h, non_blocking=True)
-        self._frame_tab_ev = torch.cuda.Event()
-        self._frame_tab_ev.record()
-        rx, ry, rw, rh = self.roi
-        rc = self._lib.fm_letterbox_preproc_batch(ptr(self._frame_tab), B, self.size[0], self.size[1],
-                                                  self.input_wh[0], self.input_wh[1], rx, ry, rw, rh, ptr(self.inp),
-                                                  stream_ptr())
-        _lib.check(rc, "fm_letterbox_preproc_batch")
-
     def detect_batch_async(self, frames):
-        """detect_async for 1..B frames at once: one letterbox launch, one conv-stack forward over the k images, one
-        decode launch per head and one batched NMS; `postprocess_batch` waits for the results.  B frames of this
-        detector's size take the batch-B engine; any other k frames (HxWx3 u8 of any sizes) the batch-k engine, each
-        frame with the letterbox and box geometry of its own size."""
+        """detect_async for 1..B frames (HxWx3 u8 of any sizes) at once: one letterbox launch, one forward of the
+        batch-k engine, one decode launch per head and one batched NMS; `postprocess_batch` waits for the results.
+        Each frame gets the letterbox and box geometry of its own size."""
         k = len(frames)
         if not 1 <= k <= self.batch:
             raise ValueError(f"expected 1 to {self.batch} frames, got {k}")
         self.frames_dev = [f if torch.is_tensor(f) else self._upload(b, f) for b, f in enumerate(frames)]
-        want = (self.size[1], self.size[0], 3)
-        if k == self.batch and all(tuple(f.shape) == want for f in self.frames_dev):
-            self.preprocess_batch(self.frames_dev)
-            heads = self.backend.forward(self.inp)
-            self.postprocess_heads_batch_async(heads)
-            return
         geom = self.preprocess_frames(self.frames_dev)
-        heads = self.engine(k).forward(self.inp[:k] if k > 1 else self.inp[0])
+        # a batch-1 input has no image dimension, in this detector and in its batch-1 engine
+        inp = self.inp if self.batch == 1 else self.inp[:k] if k > 1 else self.inp[0]
+        heads = self.engine(k).forward(inp)
         self.postprocess_heads_batch_async(heads, k, geom)
 
     def engine(self, k):
@@ -290,63 +267,60 @@ class YOLODetector(Detector):
             self._geometry[wh] = letterbox_geometry(wh, self.input_wh, self.model.LETTERBOX)
         return self._geometry[wh]
 
-    def preprocess_frames(self, frames_dev):
-        """Letterbox of k frames of any sizes (HxWx3 u8 cuda tensors) into self.inp[:k], one launch.  Uploads
-        their FmFrameGeom table (one copy from a pinned block) and returns it: the head decode reads it too."""
-        k = len(frames_dev)
-        if not 1 <= k <= self.batch:
-            raise ValueError(f"expected 1 to {self.batch} frames, got {k}")
-        rows = (_lib.FmFrameGeom * k)()
-        for r, f in zip(rows, frames_dev):
-            if f.dim() != 3 or f.shape[2] != 3 or f.dtype != torch.uint8 or not f.is_contiguous() or not f.is_cuda:
-                raise ValueError("every frame must be a contiguous HxWx3 uint8 cuda tensor")
-            h, w = f.shape[:2]
+    def _upload_geom(self, sizes, frame_ptrs):
+        """Fills one FmFrameGeom row per image, of frame size sizes[b] = (width, height) and device frame pointer
+        frame_ptrs[b] (0 when only the head decode reads the row), and uploads the rows to self._geom in one copy from
+        the pinned block; returns self._geom."""
+        rows = (_lib.FmFrameGeom * len(sizes))()
+        for r, (w, h), fp in zip(rows, sizes, frame_ptrs):
             (rx, ry, rw, rh), up, off = self.geometry((w, h))
-            r.frame, r.w, r.h = f.data_ptr(), w, h
+            r.frame, r.w, r.h = fp, w, h
             r.roi_x, r.roi_y, r.roi_w, r.roi_h = rx, ry, rw, rh
             r.size_w, r.size_h, r.off_x, r.off_y = float(up[0]), float(up[1]), float(off[0]), float(off[1])
         if self._geom_ev is not None:
             self._geom_ev.synchronize()          # the previous table upload has left the pinned block
-        nb = k * self._geom_bytes
+        nb = len(sizes) * self._geom_bytes
         C.memmove(self._geom_h.data_ptr(), C.addressof(rows), nb)
         self._geom[:nb].copy_(self._geom_h[:nb], non_blocking=True)
         self._geom_ev = torch.cuda.Event()
         self._geom_ev.record()
-        rc = self._lib.fm_letterbox_preproc_geom(ptr(self._geom), k, self.input_wh[0], self.input_wh[1],
-                                                 ptr(self.inp), stream_ptr())
-        _lib.check(rc, "fm_letterbox_preproc_geom")
         return self._geom
+
+    def preprocess_frames(self, frames_dev):
+        """Letterbox of k frames of any sizes (HxWx3 u8 cuda tensors) into self.inp[:k], one launch.  Uploads
+        their FmFrameGeom table and returns it: the head decode reads it too."""
+        k = len(frames_dev)
+        if not 1 <= k <= self.batch:
+            raise ValueError(f"expected 1 to {self.batch} frames, got {k}")
+        for f in frames_dev:
+            if f.dim() != 3 or f.shape[2] != 3 or f.dtype != torch.uint8 or not f.is_contiguous() or not f.is_cuda:
+                raise ValueError("every frame must be a contiguous HxWx3 uint8 cuda tensor")
+        geom = self._upload_geom([(f.shape[1], f.shape[0]) for f in frames_dev], [f.data_ptr() for f in frames_dev])
+        rc = self._lib.fm_letterbox_preproc_geom(ptr(geom), k, self.input_wh[0], self.input_wh[1], ptr(self.inp),
+                                                 stream_ptr())
+        _lib.check(rc, "fm_letterbox_preproc_geom")
+        return geom
 
     def postprocess_heads_batch_async(self, head_tensors, k=None, geom=None):
         """Decode + filter + NMS of k (default B) images' fp16 NHWC heads [k][H][W][(5+C)*A] ([H][W][(5+C)*A] at
         k = 1).  geom: the device FmFrameGeom table of preprocess_frames (each image's own box geometry); without it
-        every image has this detector's size."""
+        every image has this detector's size, and k rows of that size are uploaded."""
         s = stream_ptr()
         B, k0 = self.batch, self.num_candidates
         k = B if k is None else k
+        if geom is None:
+            geom = self._upload_geom([self.size] * k, [0] * k)
         self._k = k
         self._counter.zero_()
         lib = self._lib
         for hd, t in zip(self.heads, head_tensors):
             assert t.is_contiguous() and t.dtype == torch.float16 and t.numel() % k == 0
-            if geom is None:
-                rc = lib.fm_yolo_decode_filter_batch(ptr(t), k, t.numel() // k, 1, 1, hd['w'], hd['h'], hd['na'],
-                                                     C.byref(hd['head']), self.model.NUM_CLASSES, self.input_wh[0],
-                                                     self.input_wh[1], 1 if self.model.NEW_COORDS else 0, hd['base'],
-                                                     k0, ptr(self._label_mask_dev), float(self.conf_thresh),
-                                                     float(self.upscaled_sz[0]), float(self.upscaled_sz[1]),
-                                                     float(self.bbox_offset[0]), float(self.bbox_offset[1]),
-                                                     ptr(self._dense), ptr(self._keys), ptr(self._counter),
-                                                     self.key_cap, s)
-                _lib.check(rc, "fm_yolo_decode_filter_batch")
-            else:
-                rc = lib.fm_yolo_decode_filter_geom(ptr(t), k, t.numel() // k, 1, 1, hd['w'], hd['h'], hd['na'],
-                                                    C.byref(hd['head']), self.model.NUM_CLASSES, self.input_wh[0],
-                                                    self.input_wh[1], 1 if self.model.NEW_COORDS else 0, hd['base'],
-                                                    k0, ptr(self._label_mask_dev), float(self.conf_thresh), ptr(geom),
-                                                    ptr(self._dense), ptr(self._keys), ptr(self._counter),
-                                                    self.key_cap, s)
-                _lib.check(rc, "fm_yolo_decode_filter_geom")
+            rc = lib.fm_yolo_decode_filter_geom(ptr(t), k, t.numel() // k, 1, 1, hd['w'], hd['h'], hd['na'],
+                                                C.byref(hd['head']), self.model.NUM_CLASSES, self.input_wh[0],
+                                                self.input_wh[1], 1 if self.model.NEW_COORDS else 0, hd['base'], k0,
+                                                ptr(self._label_mask_dev), float(self.conf_thresh), ptr(geom),
+                                                ptr(self._dense), ptr(self._keys), ptr(self._counter), self.key_cap, s)
+            _lib.check(rc, "fm_yolo_decode_filter_geom")
         meta = self._out_meta
         rc = lib.fm_diou_nms_filter_batch(k, ptr(self._keys), ptr(self._dense), k0, ptr(self._counter), self.key_cap,
                                           float(self.nms_thresh), float(self.max_area), float(self.min_aspect_ratio),
@@ -365,28 +339,12 @@ class YOLODetector(Detector):
         `postprocess` orders one frame's detections.  An overflow raises and names image b as names[b] (default
         'image b')."""
         self._done.synchronize()
-        B, k, md = self.batch, self._k, self.max_dets
-        meta = self._h_meta.numpy()
-        count, status, n_cand = meta[:k], meta[B:B + k], meta[2 * B:2 * B + k]
-        for b in range(k):
-            name = f"image {b}" if names is None else names[b]
-            if status[b] == 2:
-                raise RuntimeError(f"{name}: more than max_dets = {md} boxes survived NMS and the area / aspect "
-                                   "filters; raise max_dets (no silent truncation)")
-            if status[b] != 0:
-                raise RuntimeError(f"{name}: {n_cand[b]} candidates passed conf_thresh but key_cap is "
-                                   f"{self.key_cap}; raise key_cap (no silent truncation)")
-        self.last_num_candidates = [int(v) for v in n_cand]
-        out = []
-        for b in range(k):
-            n, r0 = int(count[b]), b * md
-            dets = np.zeros(n, DET_DTYPE)
-            dets['tlbr'] = self._h_tlbr.numpy()[r0:r0 + n]
-            dets['label'] = self._h_label.numpy()[r0:r0 + n]
-            dets['conf'] = self._h_conf.numpy()[r0:r0 + n]
-            out.append(dets.view(np.recarray))
+        B, k = self.batch, self._k
+        count, status, n_cand = (self._h_meta.numpy()[i * B:i * B + k].tolist() for i in range(3))
+        out = [self._image_dets(count[b], status[b], n_cand[b], b * self.max_dets,
+                                f"image {b}" if names is None else names[b]) for b in range(k)]
+        self.last_num_candidates = n_cand
         return out
-
 
 
 class PublicDetector(Detector):

@@ -91,8 +91,8 @@ class MultiCameraMOT:
         if len(feature_extractor_cfgs) != len(class_ids):
             raise ValueError('Number of feature extractors must match length of class IDs')
 
-        # N frames of the first camera's size take the batch-N engine with that size's geometry; any other set of
-        # frames carries each frame's own geometry
+        # a detector call over k cameras' frames runs the batch-k engine (the batch-N one at k = N), each frame with the
+        # geometry of its own size
         self.detector = YOLODetector(self.sizes[0], self.class_ids, batch=N, **vars(yolo_detector_cfg))
         # one extractor per class as in MOT; its crop capacity holds every camera's crops
         self.extractors = []

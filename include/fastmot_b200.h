@@ -179,10 +179,6 @@ typedef struct FmFrameGeom {
  * layout 0: fp32 planar CHW (the reference's TensorRT input); layout 1: fp16 NHWC, C padded to 8 (16 bytes per pixel). */
 int fm_letterbox_preproc(const unsigned char* frame, int src_w, int src_h, int dst_w, int dst_h, int roi_x, int roi_y,
                          int roi_w, int roi_h, int layout, void* out, void* stream);
-/* fm_letterbox_preproc (layout 1) of `batch` frames of one size in one launch: frames is a DEVICE array of batch
- * frame pointers; out is fp16 [batch][dst_h][dst_w][8], image b bit-identical to the one-frame call on frames[b]. */
-int fm_letterbox_preproc_batch(const unsigned char* const* frames, int batch, int src_w, int src_h, int dst_w,
-                               int dst_h, int roi_x, int roi_y, int roi_w, int roi_h, void* out, void* stream);
 /* fm_letterbox_preproc (layout 1) of `batch` frames of any sizes in one launch: geom is a DEVICE array of batch rows
  * (frame, w, h and roi_* are read; every roi_w, roi_h > 0); out is fp16 [batch][dst_h][dst_w][8], image b
  * bit-identical to the one-frame call on geom[b]'s frame, size and ROI. */
@@ -196,13 +192,10 @@ int fm_letterbox_preproc_geom(const FmFrameGeom* geom, int batch, int dst_w, int
  * the OSNet 7x7 stem, fm_osnet_stem). */
 int fm_roi_resize_norm(const unsigned char* frame, int src_w, int src_h, const double* tlbrs, const int* n_dev,
                        int n_max, int out_w, int out_h, int layout, void* out, void* stream);
-/* fm_roi_resize_norm over several frames of one size in one launch: crop i (tlbrs[i]) is cut from
- * frames[frame_idx[i]] (frames: DEVICE array of frame pointers, frame_idx: device int32 [n]); each crop is
- * bit-identical to the one-frame call on its own frame and box. */
-int fm_roi_resize_norm_multi(const unsigned char* const* frames, const int* frame_idx, int src_w, int src_h,
-                             const double* tlbrs, int n, int out_w, int out_h, int layout, void* out, void* stream);
-/* fm_roi_resize_norm_multi over frames of any sizes: crop i is cut from geom[frame_idx[i]].frame, clamped to and
- * addressed with that row's w and h (geom: DEVICE FmFrameGeom array; the ROI and scale fields are not read). */
+/* fm_roi_resize_norm over several frames of any sizes in one launch: crop i (tlbrs[i]) is cut from
+ * geom[frame_idx[i]].frame, clamped to and addressed with that row's w and h (geom: DEVICE FmFrameGeom array, the ROI
+ * and scale fields are not read; frame_idx: device int32 [n]); each crop is bit-identical to the one-frame call on its
+ * own frame and box. */
 int fm_roi_resize_norm_geom(const FmFrameGeom* geom, const int* frame_idx, const double* tlbrs, int n, int out_w,
                             int out_h, int layout, void* out, void* stream);
 
@@ -216,19 +209,11 @@ int fm_yolo_decode_filter(const void* head_out, int is_fp16, int nhwc, int yolo_
                           int cand_base, const unsigned char* label_mask, double conf_thresh, float size_w,
                           float size_h, float off_x, float off_y, float* dense, unsigned long long* keys,
                           int* counter, int key_cap, void* stream);
-/* fm_yolo_decode_filter for one head of `batch` images in one launch.  Image b reads head_out + b * head_stride
- * elements and owns dense rows [b * cand_stride, (b + 1) * cand_stride) (its candidate cand_base + idx at row
+/* fm_yolo_decode_filter for one head of `batch` images in one launch, with image b's size_w, size_h, off_x, off_y read
+ * from geom[b] (DEVICE FmFrameGeom array of batch rows).  Image b reads head_out + b * head_stride elements and owns
+ * dense rows [b * cand_stride, (b + 1) * cand_stride) (its candidate cand_base + idx at row
  * b * cand_stride + cand_base + idx), keys[b * key_cap .. + key_cap) and counters[b]: its keys and rows are the
- * one-image call's on its head slice. */
-int fm_yolo_decode_filter_batch(const void* head_out, int batch, long long head_stride, int is_fp16, int nhwc,
-                                int yolo_w, int yolo_h, int num_anchors, const FmYoloHead* h_head, int num_classes,
-                                int input_w, int input_h, int new_coords, int cand_base, int cand_stride,
-                                const unsigned char* label_mask, double conf_thresh, float size_w, float size_h,
-                                float off_x, float off_y, float* dense, unsigned long long* keys, int* counters,
-                                int key_cap, void* stream);
-/* fm_yolo_decode_filter_batch with image b's size_w, size_h, off_x, off_y read from geom[b] (DEVICE FmFrameGeom array
- * of batch rows): image b's keys and rows are the one-image call's on its head slice with its own geometry, in the
- * segment layout fm_diou_nms_filter_batch reads. */
+ * one-image call's on its head slice with its own geometry. */
 int fm_yolo_decode_filter_geom(const void* head_out, int batch, long long head_stride, int is_fp16, int nhwc,
                                int yolo_w, int yolo_h, int num_anchors, const FmYoloHead* h_head, int num_classes,
                                int input_w, int input_h, int new_coords, int cand_base, int cand_stride,
@@ -245,7 +230,7 @@ int fm_diou_nms_filter(unsigned long long* keys, const float* dense, const int* 
                        double nms_thresh, double max_area, double min_aspect_ratio, unsigned long long* mask,
                        int max_out, double* out_tlbr, long long* out_label, double* out_conf, int* out_count,
                        int* status, void* stream);
-/* fm_diou_nms_filter for `batch` images in one call, on the segments fm_yolo_decode_filter_batch wrote: a box only
+/* fm_diou_nms_filter for `batch` images in one call, on the segments fm_yolo_decode_filter_geom wrote: a box only
  * suppresses boxes of its own image and class.  mask: batch x fm_nms_mask_bytes(key_cap) bytes (image b's rows at
  * b x that size; only its first counters[b] rows are written).  Outputs: image b's detections at rows
  * [b * max_out, b * max_out + out_count[b]) of out_tlbr / out_label / out_conf; status[b] as above. */

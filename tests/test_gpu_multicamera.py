@@ -279,3 +279,32 @@ def test_shared_engine_launch_by_launch_heads_and_memory(gcase, monkeypatch):
     for a, b in zip(eng3.heads, alone.heads):
         assert a.shape == b.shape
         assert torch.equal(_bits(a), _bits(b))
+
+
+@pytest.mark.parametrize("name", MODELS)
+def test_frames_of_the_detectors_own_size_run_the_batch_b_engine(name, monkeypatch):
+    """B = 2 different frames of the detector's own size through detect_batch_async: the batch-2 engine runs them (no
+    batch-k engine is built), each image's letterbox equals fm_letterbox_preproc on its frame bit for bit, and each
+    image's keys, candidate rows and detections equal the one-image decode + NMS of its head slice."""
+    from test_gpu_yolo_zoo import _per_image_equals_one_image
+    from fastmot_b200 import _lib
+    from fastmot_b200.detector import YOLODetector
+    from fastmot_b200.devmem import ptr, stream_ptr
+    from fastmot_b200.synth import SyntheticScene
+    _synth_env(monkeypatch, name)
+    size = SIZES[0]
+    det = YOLODetector(size, (0,), name, batch=2)
+    frames = [torch.as_tensor(SyntheticScene(200, size=size, seed=5 + 7 * b).frame(b)).cuda() for b in range(2)]
+    det.detect_batch_async(frames)
+    torch.cuda.synchronize()
+    assert sorted(det._engines) == [2]
+    lib = _lib.load()
+    rx, ry, rw, rh = det.roi
+    for b, f in enumerate(frames):
+        one = torch.zeros_like(det.inp[0])
+        _lib.check(lib.fm_letterbox_preproc(ptr(f), size[0], size[1], det.input_wh[0], det.input_wh[1], rx, ry, rw, rh,
+                                            1, ptr(one), stream_ptr()), "fm_letterbox_preproc")
+        torch.cuda.synchronize()
+        assert torch.equal(det.inp[b].view(torch.int16), one.view(torch.int16)), (name, b)
+    assert not torch.equal(det.inp[0], det.inp[1])
+    _per_image_equals_one_image(det, det.backend.heads, [size] * 2, name)

@@ -140,7 +140,7 @@ class BatchCase:
         self.det = YOLODetector((1920, 1080), classes, name, engine=self.eng, batch=B)
         self.det1 = YOLODetector((1920, 1080), classes, name, engine=NS(heads_nhwc=True))
         self.frames = [torch.as_tensor(SyntheticScene(200, seed=3 + 7 * b).frame(b)).cuda() for b in range(B)]
-        self.det.preprocess_batch(self.frames)
+        self.det.preprocess_frames(self.frames)
         self.eng.forward(self.det.inp)
         torch.cuda.synchronize()
 
@@ -149,7 +149,8 @@ class BatchCase:
         torch.cuda.empty_cache()
 
 
-@pytest.fixture(scope="module", params=['YOLOv4Tiny', 'YOLOv4CSP'])
+# plain resize with old head coordinates (tiny-416, YOLOv4-512) and letterbox with new ones (csp-640, P5-896)
+@pytest.fixture(scope="module", params=['YOLOv4Tiny', 'YOLOv4CSP', 'YOLOv4', 'YOLOv4P5'])
 def bcase(request):
     c = BatchCase(request.param)
     yield c
@@ -350,7 +351,7 @@ def _boxes(n, seed):
 
 
 def test_shared_reid_batch():
-    """3 streams x 67 crops (201, not a multiple of 8): every crop of fm_roi_resize_norm_multi equals the one-frame
+    """3 streams x 67 crops (201, not a multiple of 8): every crop of fm_roi_resize_norm_geom equals the one-frame
     crop bit for bit; the shared forward's per-stream rows agree with one forward per stream (<= 5e-3 abs) and are
     views of the shared output; every launch of the shared forward passes the float64 check."""
     from test_gpu_osnet_ops import run_launch_by_launch
