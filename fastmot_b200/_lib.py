@@ -81,7 +81,11 @@ class FmYoloHead(C.Structure):
 
 class FmFrameGeom(C.Structure):
     _fields_ = [("frame", c_p), ("w", c_i), ("h", c_i), ("roi_x", c_i), ("roi_y", c_i), ("roi_w", c_i),
-                ("roi_h", c_i), ("size_w", c_f), ("size_h", c_f), ("off_x", c_f), ("off_y", c_f)]
+                ("roi_h", c_i), ("size_w", c_f), ("size_h", c_f), ("off_x", c_f), ("off_y", c_f),
+                ("uv", c_p), ("pitch", c_i), ("uv_pitch", c_i), ("format", c_i)]
+
+
+FM_PIX_BGR, FM_PIX_NV12 = 0, 1
 
 
 # name -> (restype, argtypes); kept in one table so tests can check it against the header
@@ -108,6 +112,8 @@ SIGNATURES = {
     "fm_assoc_cascade_out_ints": (c_ll, [c_i]),
     "fm_letterbox_preproc": (c_i, [c_p, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_p, c_p]),
     "fm_roi_resize_norm": (c_i, [c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p]),
+    "fm_letterbox_preproc_nv12": (c_i, [c_p, c_p, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_p, c_p]),
+    "fm_roi_resize_norm_nv12": (c_i, [c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p]),
     "fm_letterbox_preproc_geom": (c_i, [c_p, c_i, c_i, c_i, c_p, c_p]),
     "fm_roi_resize_norm_geom": (c_i, [c_p, c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p]),
     "fm_yolo_decode_filter_geom": (c_i, [c_p, c_i, c_ll, c_i, c_i, c_i, c_i, c_i, C.POINTER(FmYoloHead), c_i, c_i,
@@ -118,6 +124,8 @@ SIGNATURES = {
                                      c_d, c_f, c_f, c_f, c_f, c_p, c_p, c_p, c_i, c_p]),
     "fm_gray_half": (c_i, [c_p, c_i, c_i, c_p, c_p, c_p]),
     "fm_gray_resize": (c_i, [c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_p]),
+    "fm_gray_half_nv12": (c_i, [c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p, c_p]),
+    "fm_gray_resize_nv12": (c_i, [c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p, c_i, c_i, c_p]),
     "fm_pyr_level": (c_i, [c_p, c_i, c_i, c_p, c_p]),
     "fm_scharr": (c_i, [c_p, c_i, c_i, c_p, c_p]),
     "fm_bg_small": (c_i, [c_p, c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_p]),
@@ -136,6 +144,8 @@ SIGNATURES = {
     "fm_flow_plan_destroy": (None, [c_p]),
     "fm_flow_preprocess": (c_i, [c_p, c_p, c_i, c_p]),
     "fm_flow_predict": (c_i, [c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_p]),
+    "fm_flow_preprocess_nv12": (c_i, [c_p, c_p, c_p, c_i, c_i, c_i, c_p]),
+    "fm_flow_predict_nv12": (c_i, [c_p, c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p, c_p, c_p]),
     "fm_conv2d_simt": (c_i, [C.POINTER(FmConvDesc), c_p, c_p, c_p, c_p, c_p, c_p]),
     "fm_maxpool": (c_i, [c_p, c_p, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_p]),
     "fm_maxpool_pad": (c_i, [c_p, c_p, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_p]),

@@ -1,5 +1,5 @@
 // KLT image pyramid kernels (byte work, HBM/L2-bound): BGR->gray + 0.5x box mean in one pass, BGR->gray + an
-// INTER_LINEAR resize to any optical-flow size, 5-tap Gaussian pyrDown, int16 Scharr derivatives, 0.1x background
+// INTER_LINEAR resize to any optical-flow size (both also reading NV12 frames in place, pixel_src.cuh), 5-tap Gaussian pyrDown, int16 Scharr derivatives, 0.1x background
 // image + mask.
 //
 // Reference: fastmot/flow.py:121-133, 153-154, 187-189 (cv2.cvtColor / cv2.resize) and the pyramid that
@@ -7,28 +7,46 @@
 // calcScharrDeriv).  Fixed-point formulas restated in SURVEY.md Appendix C.
 #include "common.cuh"
 #include "../../include/fastmot_b200.h"
+#include "pixel_src.cuh"
 
 namespace {
 
-__device__ __forceinline__ int gray_of(const unsigned char* p) {
+__device__ __forceinline__ int gray_of(const int p[3]) {
     // OpenCV 4.13 BGR2GRAY, 15-bit fixed point (pinned against cv2.cvtColor: 0 mismatches on 1M random pixels;
     // the 14-bit constants 1868/9617/4899 quoted in SURVEY.md Appendix C differ on 0.2 % of pixels)
     return (p[0] * 3735 + p[1] * 19235 + p[2] * 9798 + 16384) >> 15;
 }
 
+// The four pixels of the 2x2 block at (x0, y0) (x1 = x0 + 1, y1 = y0 + 1 inside the frame; w and h are even).
+__device__ __forceinline__ void block_bgr(const BgrSrc& s, int x0, int y0, int x1, int y1, int a[3], int b[3],
+                                          int c[3], int d[3]) {
+    s.px(x0, y0, a); s.px(x1, y0, b); s.px(x0, y1, c); s.px(x1, y1, d);
+}
+
+// An NV12 2x2 block at even (x0, y0) is exactly one chroma sample: one UV load for the four pixels.
+__device__ __forceinline__ void block_bgr(const Nv12Src& s, int x0, int y0, int x1, int y1, int a[3], int b[3],
+                                          int c[3], int d[3]) {
+    const unsigned char* q = s.uv + (size_t)(y0 >> 1) * s.uv_pitch + x0;
+    const int U = q[0], V = q[1];
+    const unsigned char* r0 = s.y + (size_t)y0 * s.y_pitch;
+    const unsigned char* r1 = s.y + (size_t)y1 * s.y_pitch;
+    fm_yuv_to_bgr(r0[x0], U, V, a); fm_yuv_to_bgr(r0[x1], U, V, b);
+    fm_yuv_to_bgr(r1[x0], U, V, c); fm_yuv_to_bgr(r1[x1], U, V, d);
+}
+
 // One thread per 2x2 block of the full-resolution frame.
-__global__ void __launch_bounds__(256) gray_half_kernel(const unsigned char* __restrict__ frame, int w, int h,
-                                                         unsigned char* __restrict__ gray,
+template <class Src>
+__global__ void __launch_bounds__(256) gray_half_kernel(Src src, int w, int h, unsigned char* __restrict__ gray,
                                                          unsigned char* __restrict__ small, int sw, int sh) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x;  // small coords
     const int y = blockIdx.y;
     if (x >= sw || y >= sh) return;
     const int x0 = 2 * x, y0 = 2 * y;
     const int x1 = min(x0 + 1, w - 1), y1 = min(y0 + 1, h - 1);
-    const unsigned char* r0 = frame + (size_t)y0 * w * 3;
-    const unsigned char* r1 = frame + (size_t)y1 * w * 3;
-    const int a = gray_of(r0 + x0 * 3), b = gray_of(r0 + x1 * 3);
-    const int c = gray_of(r1 + x0 * 3), d = gray_of(r1 + x1 * 3);
+    int pa[3], pb[3], pc[3], pd[3];
+    block_bgr(src, x0, y0, x1, y1, pa, pb, pc, pd);
+    const int a = gray_of(pa), b = gray_of(pb);
+    const int c = gray_of(pc), d = gray_of(pd);
     gray[(size_t)y0 * w + x0] = a;
     gray[(size_t)y0 * w + x1] = b;
     gray[(size_t)y1 * w + x0] = c;
@@ -36,12 +54,14 @@ __global__ void __launch_bounds__(256) gray_half_kernel(const unsigned char* __r
     small[(size_t)y * sw + x] = (a + b + c + d + 2) >> 2;  // cv2.resize INTER_LINEAR at exactly 0.5x
 }
 
-__global__ void __launch_bounds__(256) gray_kernel(const unsigned char* __restrict__ frame, int w, int h,
-                                                    unsigned char* __restrict__ gray) {
+template <class Src>
+__global__ void __launch_bounds__(256) gray_kernel(Src src, int w, int h, unsigned char* __restrict__ gray) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y;
     if (x >= w || y >= h) return;
-    gray[(size_t)y * w + x] = gray_of(frame + ((size_t)y * w + x) * 3);
+    int p[3];
+    src.px(x, y, p);
+    gray[(size_t)y * w + x] = gray_of(p);
 }
 
 // cv2.resize(src, (dw, dh)) INTER_LINEAR for u8 at a downscale (dw <= sw, dh <= sh): OpenCV's generic resize with
@@ -138,26 +158,54 @@ __global__ void bg_small_kernel(const unsigned char* __restrict__ gray, const in
 
 }  // namespace
 
-extern "C" int fm_gray_half(const unsigned char* frame, int w, int h, unsigned char* gray, unsigned char* small,
-                            void* stream) {
+namespace {
+template <class Src>
+int gray_half_launch(const char* name, Src src, int w, int h, unsigned char* gray, unsigned char* small, void* stream) {
     const int sw = (w + 1) / 2, sh = (h + 1) / 2;
     FM_REQUIRE(w % 2 == 0 && h % 2 == 0, "fm_gray_half: frame size must be even (0.5x resize = 2x2 mean)");
     dim3 grid(fm_cdiv(sw, 256), sh);
-    gray_half_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(frame, w, h, gray, small, sw, sh);
-    FM_CHECK_LAUNCH("fm_gray_half");
+    gray_half_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(src, w, h, gray, small, sw, sh);
+    FM_CHECK_LAUNCH(name);
     return FM_OK;
+}
+
+template <class Src>
+int gray_resize_launch(const char* name, Src src, int w, int h, unsigned char* gray, unsigned char* small, int sw,
+                       int sh, void* stream) {
+    FM_REQUIRE(w > 0 && h > 0 && sw > 0 && sh > 0 && sw <= w && sh <= h,
+               "fm_gray_resize: the optical-flow image must be non-empty and no larger than the frame");
+    gray_kernel<<<dim3(fm_cdiv(w, 256), h), 256, 0, (cudaStream_t)stream>>>(src, w, h, gray);
+    resize_linear_kernel<<<dim3(fm_cdiv(sw, 256), sh), 256, 0, (cudaStream_t)stream>>>(
+        gray, w, h, small, sw, sh, 1.0 / ((double)sw / w), 1.0 / ((double)sh / h));
+    fm_count_launches(1);
+    FM_CHECK_LAUNCH(name);
+    return FM_OK;
+}
+}  // namespace
+
+extern "C" int fm_gray_half(const unsigned char* frame, int w, int h, unsigned char* gray, unsigned char* small,
+                            void* stream) {
+    return gray_half_launch("fm_gray_half", BgrSrc{frame, w}, w, h, gray, small, stream);
+}
+
+extern "C" int fm_gray_half_nv12(const unsigned char* y, const unsigned char* uv, int y_pitch, int uv_pitch, int w,
+                                 int h, unsigned char* gray, unsigned char* small, void* stream) {
+    FM_REQUIRE(fm_nv12_ok(y, uv, y_pitch, uv_pitch, w, h),
+               "fm_gray_half_nv12: NV12 needs even w, h > 0, both planes and pitches >= w");
+    return gray_half_launch("fm_gray_half_nv12", Nv12Src{y, uv, y_pitch, uv_pitch}, w, h, gray, small, stream);
 }
 
 extern "C" int fm_gray_resize(const unsigned char* frame, int w, int h, unsigned char* gray, unsigned char* small,
                               int sw, int sh, void* stream) {
-    FM_REQUIRE(w > 0 && h > 0 && sw > 0 && sh > 0 && sw <= w && sh <= h,
-               "fm_gray_resize: the optical-flow image must be non-empty and no larger than the frame");
-    gray_kernel<<<dim3(fm_cdiv(w, 256), h), 256, 0, (cudaStream_t)stream>>>(frame, w, h, gray);
-    resize_linear_kernel<<<dim3(fm_cdiv(sw, 256), sh), 256, 0, (cudaStream_t)stream>>>(
-        gray, w, h, small, sw, sh, 1.0 / ((double)sw / w), 1.0 / ((double)sh / h));
-    fm_count_launches(1);
-    FM_CHECK_LAUNCH("fm_gray_resize");
-    return FM_OK;
+    return gray_resize_launch("fm_gray_resize", BgrSrc{frame, w}, w, h, gray, small, sw, sh, stream);
+}
+
+extern "C" int fm_gray_resize_nv12(const unsigned char* y, const unsigned char* uv, int y_pitch, int uv_pitch, int w,
+                                   int h, unsigned char* gray, unsigned char* small, int sw, int sh, void* stream) {
+    FM_REQUIRE(fm_nv12_ok(y, uv, y_pitch, uv_pitch, w, h),
+               "fm_gray_resize_nv12: NV12 needs even w, h > 0, both planes and pitches >= w");
+    return gray_resize_launch("fm_gray_resize_nv12", Nv12Src{y, uv, y_pitch, uv_pitch}, w, h, gray, small, sw, sh,
+                              stream);
 }
 
 extern "C" int fm_pyr_level(const unsigned char* src, int sw, int sh, unsigned char* dst, void* stream) {

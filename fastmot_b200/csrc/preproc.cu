@@ -4,13 +4,15 @@
 //   fm_roi_resize_norm   : per-detection crop + OpenCV-style fixed-point bilinear resize to 128x256 + ImageNet
 //                          normalisation, all crops in one launch (fastmot/feature_extractor.py:48-60, 84-98;
 //                          fastmot/utils/rect.py:92-97)
-// The *_geom entries read each frame's pointer, size (and, for the letterbox, ROI) from a device FmFrameGeom table
-// (one grid slice per frame, or one frame index per crop), so one launch covers several frames of any sizes; every
-// pixel is computed by the same kernel body as in the one-frame entries.
+// The *_geom entries read each frame's pointer, size, pixel format (and, for the letterbox, ROI) from a device
+// FmFrameGeom table (one grid slice per frame, or one frame index per crop), so one launch covers several frames of
+// any sizes and formats; every pixel is computed by the same body as in the one-frame entries.  The *_nv12 entries
+// read an NV12 frame in place (pixel_src.cuh): each bilinear tap is converted to BGR before it is interpolated.
 // Outputs are either fp32 planar CHW (the reference's TensorRT input layout; used for parity tests) or fp16
 // NHWC with C padded to 8 (one 16-byte chunk per pixel; what the conv engine consumes).
 #include "common.cuh"
 #include "../../include/fastmot_b200.h"
+#include "pixel_src.cuh"
 
 namespace {
 
@@ -38,23 +40,10 @@ __device__ __forceinline__ void store_px(void* out, int H, int W, int y, int x, 
     }
 }
 
-// geom != nullptr: image blockIdx.z takes its frame, size and ROI from geom[blockIdx.z] and writes the blockIdx.z-th
-// NHWC8 image of out
-template <int LAYOUT>
-__global__ void __launch_bounds__(256) letterbox_kernel(const unsigned char* __restrict__ frame,
-                                                         const FmFrameGeom* __restrict__ geom, int src_w,
-                                                         int src_h, int dst_w, int dst_h, int roi_x, int roi_y,
-                                                         int roi_w, int roi_h, void* __restrict__ out) {
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    const int y = blockIdx.y;
-    if (x >= dst_w) return;
-    if (geom != nullptr) {
-        const FmFrameGeom& g = geom[blockIdx.z];
-        frame = g.frame;
-        src_w = g.w; src_h = g.h;
-        roi_x = g.roi_x; roi_y = g.roi_y; roi_w = g.roi_w; roi_h = g.roi_h;
-        out = (__half*)out + (size_t)blockIdx.z * dst_h * dst_w * 8;
-    }
+// One output pixel (x, y) of the letterbox of a src_w x src_h frame read through `src`.
+template <int LAYOUT, class Src>
+__device__ __forceinline__ void letterbox_px(const Src& src, int src_w, int src_h, int dst_w, int dst_h, int roi_x,
+                                             int roi_y, int roi_w, int roi_h, void* out, int x, int y) {
     const int rx = x - roi_x, ry = y - roi_y;
     if (rx < 0 || ry < 0 || rx >= roi_w || ry >= roi_h) {
         store_px<LAYOUT>(out, dst_h, dst_w, y, x, 0.5f, 0.5f, 0.5f);  // detector.py:318
@@ -68,10 +57,12 @@ __global__ void __launch_bounds__(256) letterbox_kernel(const unsigned char* __r
     const int x0 = (int)floor(sx), y0 = (int)floor(sy);
     const int x1 = min(x0 + 1, src_w - 1), y1 = min(y0 + 1, src_h - 1);
     const double fx = sx - x0, fy = sy - y0;
-    const unsigned char* p00 = frame + ((size_t)y0 * src_w + x0) * 3;
-    const unsigned char* p01 = frame + ((size_t)y0 * src_w + x1) * 3;
-    const unsigned char* p10 = frame + ((size_t)y1 * src_w + x0) * 3;
-    const unsigned char* p11 = frame + ((size_t)y1 * src_w + x1) * 3;
+    // each tap is a BGR pixel before interpolation (an NV12 tap is converted with its own chroma)
+    int p00[3], p01[3], p10[3], p11[3];
+    src.px(x0, y0, p00);
+    src.px(x1, y0, p01);
+    src.px(x0, y1, p10);
+    src.px(x1, y1, p11);
     float v[3];
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
@@ -81,6 +72,30 @@ __global__ void __launch_bounds__(256) letterbox_kernel(const unsigned char* __r
         v[c] = (float)(val * (1.0 / 255.0));                      // cp.multiply(u8, 1/255.) -> f32
     }
     store_px<LAYOUT>(out, dst_h, dst_w, y, x, v[2], v[1], v[0]);  // BGR -> RGB
+}
+
+template <int LAYOUT, class Src>
+__global__ void __launch_bounds__(256) letterbox_kernel(Src src, int src_w, int src_h, int dst_w, int dst_h, int roi_x,
+                                                         int roi_y, int roi_w, int roi_h, void* __restrict__ out) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    if (x >= dst_w) return;
+    letterbox_px<LAYOUT>(src, src_w, src_h, dst_w, dst_h, roi_x, roi_y, roi_w, roi_h, out, x, blockIdx.y);
+}
+
+// image blockIdx.z takes its frame (BGR or NV12), size and ROI from geom[blockIdx.z] and writes the blockIdx.z-th
+// NHWC8 image of out
+__global__ void __launch_bounds__(256) letterbox_geom_kernel(const FmFrameGeom* __restrict__ geom, int dst_w,
+                                                              int dst_h, void* __restrict__ out) {
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    if (x >= dst_w) return;
+    const FmFrameGeom& g = geom[blockIdx.z];
+    out = (__half*)out + (size_t)blockIdx.z * dst_h * dst_w * 8;
+    if (g.format == FM_PIX_NV12)
+        letterbox_px<1>(Nv12Src{g.frame, g.uv, g.pitch ? g.pitch : g.w, g.uv_pitch ? g.uv_pitch : g.w}, g.w, g.h,
+                        dst_w, dst_h, g.roi_x, g.roi_y, g.roi_w, g.roi_h, out, x, blockIdx.y);
+    else
+        letterbox_px<1>(BgrSrc{g.frame, g.w}, g.w, g.h, dst_w, dst_h, g.roi_x, g.roi_y, g.roi_w, g.roi_h, out, x,
+                        blockIdx.y);
 }
 
 // OpenCV INTER_LINEAR for 8-bit: 11-bit fixed-point coefficients, horizontal pass in int, vertical pass
@@ -96,25 +111,10 @@ __device__ __forceinline__ void cv_coef(int d, double scale, int ssize, int& s, 
     a1 = (int)rintf(f * 2048.f);
 }
 
-// geom != nullptr: crop i is cut from geom[frame_idx[i]].frame, with that frame's own width and height
-template <int LAYOUT>
-__global__ void __launch_bounds__(128) roi_resize_norm_kernel(const unsigned char* __restrict__ frame,
-                                                               const FmFrameGeom* __restrict__ geom,
-                                                               const int* __restrict__ frame_idx, int src_w,
-                                                               int src_h, const double* __restrict__ tlbrs,
-                                                               const int* __restrict__ n_ptr, int n_max, int out_w,
-                                                               int out_h, void* __restrict__ out) {
-    const int crop = blockIdx.z;
-    const int n = n_ptr ? min(*n_ptr, n_max) : n_max;
-    if (crop >= n) return;
-    if (geom != nullptr) {
-        const FmFrameGeom& g = geom[frame_idx[crop]];
-        frame = g.frame;
-        src_w = g.w; src_h = g.h;
-    }
-    const int x = blockIdx.x * blockDim.x + threadIdx.x;
-    const int y = blockIdx.y;
-    if (x >= out_w) return;
+// Crop `crop` of a src_w x src_h frame read through `src`, output pixel (x, y).
+template <int LAYOUT, class Src>
+__device__ __forceinline__ void roi_px(const Src& src, int src_w, int src_h, const double* __restrict__ tlbrs, int crop,
+                                       int out_w, int out_h, void* __restrict__ out, int x, int y) {
     // multi_crop (rect.py:92-97): truncate toward zero, clamp lower bound to 0; numpy slicing clamps the upper
     const double* b = tlbrs + (size_t)crop * 4;
     int cx0 = max((int)b[0], 0), cy0 = max((int)b[1], 0);
@@ -125,15 +125,19 @@ __global__ void __launch_bounds__(128) roi_resize_norm_kernel(const unsigned cha
     cv_coef(x, (double)cw / out_w, cw, sx, a0, a1);
     cv_coef(y, (double)ch / out_h, ch, sy, b0, b1);
     const int sx1 = min(sx + 1, cw - 1), sy1 = min(sy + 1, ch - 1);
-    const unsigned char* r0 = frame + ((size_t)(cy0 + sy) * src_w + cx0) * 3;
-    const unsigned char* r1 = frame + ((size_t)(cy0 + sy1) * src_w + cx0) * 3;
+    // each tap is a BGR pixel before interpolation (an NV12 tap is converted with its own chroma)
+    int p00[3], p01[3], p10[3], p11[3];
+    src.px(cx0 + sx, cy0 + sy, p00);
+    src.px(cx0 + sx1, cy0 + sy, p01);
+    src.px(cx0 + sx, cy0 + sy1, p10);
+    src.px(cx0 + sx1, cy0 + sy1, p11);
     float v[3];
     const float mean[3] = {0.406f, 0.456f, 0.485f};   // indexed by BGR channel
     const float stdv[3] = {0.225f, 0.224f, 0.229f};
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-        int h0 = r0[sx * 3 + c] * a0 + r0[sx1 * 3 + c] * a1;
-        int h1 = r1[sx * 3 + c] * a0 + r1[sx1 * 3 + c] * a1;
+        int h0 = p00[c] * a0 + p01[c] * a1;
+        int h1 = p10[c] * a0 + p11[c] * a1;
         int px = (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2;
         px = min(max(px, 0), 255);
         v[c] = (float)(((double)px / 255.0 - (double)mean[c]) / (double)stdv[c]);
@@ -144,41 +148,106 @@ __global__ void __launch_bounds__(128) roi_resize_norm_kernel(const unsigned cha
     store_px<LAYOUT>(o, out_h, out_w, y, x, v[2], v[1], v[0]);
 }
 
+template <int LAYOUT, class Src>
+__global__ void __launch_bounds__(128) roi_resize_norm_kernel(Src src, int src_w, int src_h,
+                                                               const double* __restrict__ tlbrs,
+                                                               const int* __restrict__ n_ptr, int n_max, int out_w,
+                                                               int out_h, void* __restrict__ out) {
+    const int crop = blockIdx.z;
+    const int n = n_ptr ? min(*n_ptr, n_max) : n_max;
+    if (crop >= n) return;
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    if (x >= out_w) return;
+    roi_px<LAYOUT>(src, src_w, src_h, tlbrs, crop, out_w, out_h, out, x, blockIdx.y);
+}
+
+// crop i is cut from geom[frame_idx[i]]'s frame (BGR or NV12), with that frame's own width and height
+template <int LAYOUT>
+__global__ void __launch_bounds__(128) roi_resize_norm_geom_kernel(const FmFrameGeom* __restrict__ geom,
+                                                                    const int* __restrict__ frame_idx,
+                                                                    const double* __restrict__ tlbrs, int n, int out_w,
+                                                                    int out_h, void* __restrict__ out) {
+    const int crop = blockIdx.z;
+    if (crop >= n) return;
+    const int x = blockIdx.x * blockDim.x + threadIdx.x;
+    if (x >= out_w) return;
+    const FmFrameGeom& g = geom[frame_idx[crop]];
+    if (g.format == FM_PIX_NV12)
+        roi_px<LAYOUT>(Nv12Src{g.frame, g.uv, g.pitch ? g.pitch : g.w, g.uv_pitch ? g.uv_pitch : g.w}, g.w, g.h,
+                       tlbrs, crop, out_w, out_h, out, x, blockIdx.y);
+    else
+        roi_px<LAYOUT>(BgrSrc{g.frame, g.w}, g.w, g.h, tlbrs, crop, out_w, out_h, out, x, blockIdx.y);
+}
+
 }  // namespace
 
-extern "C" int fm_letterbox_preproc(const unsigned char* frame, int src_w, int src_h, int dst_w, int dst_h,
-                                    int roi_x, int roi_y, int roi_w, int roi_h, int layout, void* out, void* stream) {
+namespace {
+template <class Src>
+int letterbox_launch(const char* name, Src src, int src_w, int src_h, int dst_w, int dst_h, int roi_x, int roi_y,
+                     int roi_w, int roi_h, int layout, void* out, void* stream) {
     FM_REQUIRE(layout == 0 || layout == 1, "fm_letterbox_preproc: layout must be 0 (f32 CHW) or 1 (f16 NHWC8)");
     FM_REQUIRE(roi_w > 0 && roi_h > 0, "fm_letterbox_preproc: empty ROI");
     dim3 grid(fm_cdiv(dst_w, 256), dst_h);
     if (layout == 0)
-        letterbox_kernel<0><<<grid, 256, 0, (cudaStream_t)stream>>>(frame, nullptr, src_w, src_h, dst_w, dst_h, roi_x, roi_y,
+        letterbox_kernel<0><<<grid, 256, 0, (cudaStream_t)stream>>>(src, src_w, src_h, dst_w, dst_h, roi_x, roi_y,
                                                                     roi_w, roi_h, out);
     else
-        letterbox_kernel<1><<<grid, 256, 0, (cudaStream_t)stream>>>(frame, nullptr, src_w, src_h, dst_w, dst_h, roi_x, roi_y,
+        letterbox_kernel<1><<<grid, 256, 0, (cudaStream_t)stream>>>(src, src_w, src_h, dst_w, dst_h, roi_x, roi_y,
                                                                     roi_w, roi_h, out);
-    FM_CHECK_LAUNCH("fm_letterbox_preproc");
+    FM_CHECK_LAUNCH(name);
     return FM_OK;
 }
 
-extern "C" int fm_roi_resize_norm(const unsigned char* frame, int src_w, int src_h, const double* tlbrs,
-                                  const int* n_dev, int n_max, int out_w, int out_h, int layout, void* out,
-                                  void* stream) {
+template <class Src>
+int roi_launch(const char* name, Src src, int src_w, int src_h, const double* tlbrs, const int* n_dev, int n_max,
+               int out_w, int out_h, int layout, void* out, void* stream) {
     FM_REQUIRE(layout >= 0 && layout <= 2, "fm_roi_resize_norm: layout must be 0 (f32 CHW), 1 (f16 NHWC8) or 2 (f16 NHWC4, padded)");
     if (n_max <= 0) return FM_OK;
     FM_REQUIRE(n_max <= 65535, "fm_roi_resize_norm: more than 65535 crops");
     dim3 grid(fm_cdiv(out_w, 128), out_h, n_max);
     if (layout == 0)
-        roi_resize_norm_kernel<0><<<grid, 128, 0, (cudaStream_t)stream>>>(frame, nullptr, nullptr, src_w, src_h, tlbrs, n_dev, n_max,
+        roi_resize_norm_kernel<0><<<grid, 128, 0, (cudaStream_t)stream>>>(src, src_w, src_h, tlbrs, n_dev, n_max,
                                                                           out_w, out_h, out);
     else if (layout == 1)
-        roi_resize_norm_kernel<1><<<grid, 128, 0, (cudaStream_t)stream>>>(frame, nullptr, nullptr, src_w, src_h, tlbrs, n_dev, n_max,
+        roi_resize_norm_kernel<1><<<grid, 128, 0, (cudaStream_t)stream>>>(src, src_w, src_h, tlbrs, n_dev, n_max,
                                                                           out_w, out_h, out);
     else
-        roi_resize_norm_kernel<2><<<grid, 128, 0, (cudaStream_t)stream>>>(frame, nullptr, nullptr, src_w, src_h, tlbrs, n_dev, n_max,
+        roi_resize_norm_kernel<2><<<grid, 128, 0, (cudaStream_t)stream>>>(src, src_w, src_h, tlbrs, n_dev, n_max,
                                                                           out_w, out_h, out);
-    FM_CHECK_LAUNCH("fm_roi_resize_norm");
+    FM_CHECK_LAUNCH(name);
     return FM_OK;
+}
+}  // namespace
+
+extern "C" int fm_letterbox_preproc(const unsigned char* frame, int src_w, int src_h, int dst_w, int dst_h,
+                                    int roi_x, int roi_y, int roi_w, int roi_h, int layout, void* out, void* stream) {
+    return letterbox_launch("fm_letterbox_preproc", BgrSrc{frame, src_w}, src_w, src_h, dst_w, dst_h, roi_x, roi_y,
+                            roi_w, roi_h, layout, out, stream);
+}
+
+extern "C" int fm_letterbox_preproc_nv12(const unsigned char* y, const unsigned char* uv, int y_pitch, int uv_pitch,
+                                         int src_w, int src_h, int dst_w, int dst_h, int roi_x, int roi_y, int roi_w,
+                                         int roi_h, int layout, void* out, void* stream) {
+    FM_REQUIRE(fm_nv12_ok(y, uv, y_pitch, uv_pitch, src_w, src_h),
+               "fm_letterbox_preproc_nv12: NV12 needs even w, h > 0, both planes and pitches >= w");
+    return letterbox_launch("fm_letterbox_preproc_nv12", Nv12Src{y, uv, y_pitch, uv_pitch}, src_w, src_h, dst_w,
+                            dst_h, roi_x, roi_y, roi_w, roi_h, layout, out, stream);
+}
+
+extern "C" int fm_roi_resize_norm(const unsigned char* frame, int src_w, int src_h, const double* tlbrs,
+                                  const int* n_dev, int n_max, int out_w, int out_h, int layout, void* out,
+                                  void* stream) {
+    return roi_launch("fm_roi_resize_norm", BgrSrc{frame, src_w}, src_w, src_h, tlbrs, n_dev, n_max, out_w, out_h,
+                      layout, out, stream);
+}
+
+extern "C" int fm_roi_resize_norm_nv12(const unsigned char* y, const unsigned char* uv, int y_pitch, int uv_pitch,
+                                       int src_w, int src_h, const double* tlbrs, const int* n_dev, int n_max,
+                                       int out_w, int out_h, int layout, void* out, void* stream) {
+    FM_REQUIRE(fm_nv12_ok(y, uv, y_pitch, uv_pitch, src_w, src_h),
+               "fm_roi_resize_norm_nv12: NV12 needs even w, h > 0, both planes and pitches >= w");
+    return roi_launch("fm_roi_resize_norm_nv12", Nv12Src{y, uv, y_pitch, uv_pitch}, src_w, src_h, tlbrs, n_dev,
+                      n_max, out_w, out_h, layout, out, stream);
 }
 
 extern "C" int fm_letterbox_preproc_geom(const FmFrameGeom* geom, int batch, int dst_w, int dst_h, void* out,
@@ -186,8 +255,7 @@ extern "C" int fm_letterbox_preproc_geom(const FmFrameGeom* geom, int batch, int
     FM_REQUIRE(geom != nullptr, "fm_letterbox_preproc_geom: geometry table is NULL");
     FM_REQUIRE(batch > 0 && batch <= 65535, "fm_letterbox_preproc_geom: batch must be in [1, 65535]");
     dim3 grid(fm_cdiv(dst_w, 256), dst_h, batch);
-    letterbox_kernel<1><<<grid, 256, 0, (cudaStream_t)stream>>>(nullptr, geom, 0, 0, dst_w, dst_h, 0, 0, 0, 0,
-                                                                out);
+    letterbox_geom_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(geom, dst_w, dst_h, out);
     FM_CHECK_LAUNCH("fm_letterbox_preproc_geom");
     return FM_OK;
 }
@@ -200,14 +268,14 @@ extern "C" int fm_roi_resize_norm_geom(const FmFrameGeom* geom, const int* frame
     FM_REQUIRE(n <= 65535, "fm_roi_resize_norm_geom: more than 65535 crops");
     dim3 grid(fm_cdiv(out_w, 128), out_h, n);
     if (layout == 0)
-        roi_resize_norm_kernel<0><<<grid, 128, 0, (cudaStream_t)stream>>>(nullptr, geom, frame_idx, 0, 0,
-                                                                          tlbrs, nullptr, n, out_w, out_h, out);
+        roi_resize_norm_geom_kernel<0><<<grid, 128, 0, (cudaStream_t)stream>>>(geom, frame_idx, tlbrs, n, out_w, out_h,
+                                                                               out);
     else if (layout == 1)
-        roi_resize_norm_kernel<1><<<grid, 128, 0, (cudaStream_t)stream>>>(nullptr, geom, frame_idx, 0, 0,
-                                                                          tlbrs, nullptr, n, out_w, out_h, out);
+        roi_resize_norm_geom_kernel<1><<<grid, 128, 0, (cudaStream_t)stream>>>(geom, frame_idx, tlbrs, n, out_w, out_h,
+                                                                               out);
     else
-        roi_resize_norm_kernel<2><<<grid, 128, 0, (cudaStream_t)stream>>>(nullptr, geom, frame_idx, 0, 0,
-                                                                          tlbrs, nullptr, n, out_w, out_h, out);
+        roi_resize_norm_geom_kernel<2><<<grid, 128, 0, (cudaStream_t)stream>>>(geom, frame_idx, tlbrs, n, out_w, out_h,
+                                                                               out);
     FM_CHECK_LAUNCH("fm_roi_resize_norm_geom");
     return FM_OK;
 }

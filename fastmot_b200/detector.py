@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _lib, models
-from .devmem import ptr, stream_ptr, FrameUploader
+from .devmem import ptr, stream_ptr, FrameUploader, Frame, nv12_frame
 from .models.yolo import check_heads
 
 DET_DTYPE = np.dtype(
@@ -156,16 +156,30 @@ class YOLODetector(Detector):
 
     # ------------------------------------------------------------------
     def preprocess(self, frame_dev):
-        """fastmot/detector.py:289-300 on the device (frame_dev: HxWx3 u8 cuda tensor)."""
+        """fastmot/detector.py:289-300 on the device (frame_dev: HxWx3 u8 cuda tensor, or a device Frame of this
+        detector's size: an NV12 frame is read in place)."""
         rx, ry, rw, rh = self.roi
+        if isinstance(frame_dev, Frame) and frame_dev.format == "NV12":
+            if frame_dev.size != tuple(self.size):
+                raise ValueError(f"frame of size {frame_dev.size}, the detector's is {tuple(self.size)}")
+            rc = self._lib.fm_letterbox_preproc_nv12(*frame_dev.nv12_args(), self.size[0], self.size[1],
+                                                     self.input_wh[0], self.input_wh[1], rx, ry, rw, rh, 1,
+                                                     ptr(self.inp), stream_ptr())
+            _lib.check(rc, "fm_letterbox_preproc_nv12")
+            return
+        if isinstance(frame_dev, Frame):
+            frame_dev = frame_dev.y
         rc = self._lib.fm_letterbox_preproc(ptr(frame_dev), self.size[0], self.size[1], self.input_wh[0],
                                             self.input_wh[1], rx, ry, rw, rh, 1, ptr(self.inp), stream_ptr())
         _lib.check(rc, "fm_letterbox_preproc")
 
     def detect_async(self, frame):
-        """Upload (if `frame` is a host array), pre-process, run the conv stack and the whole
+        """Upload (if `frame` is a host array or a host NV12 Frame), pre-process, run the conv stack and the whole
         post-processing asynchronously; `postprocess` waits for the D result rows."""
-        self.frame_dev = frame if torch.is_tensor(frame) else self._uploader.upload(frame)
+        if isinstance(frame, Frame):
+            self.frame_dev = self._device(0, frame)
+        else:
+            self.frame_dev = frame if torch.is_tensor(frame) else self._uploader.upload(frame)
         self.preprocess(self.frame_dev)
         heads = self.backend.forward(self.inp)
         self.postprocess_heads_async(heads)
@@ -227,13 +241,13 @@ class YOLODetector(Detector):
 
     # ------------------------------------------------------------------ batch > 1
     def detect_batch_async(self, frames):
-        """detect_async for 1..B frames (HxWx3 u8 of any sizes) at once: one letterbox launch, one forward of the
-        batch-k engine, one decode launch per head and one batched NMS; `postprocess_batch` waits for the results.
-        Each frame gets the letterbox and box geometry of its own size."""
+        """detect_async for 1..B frames (HxWx3 u8 of any sizes, or Frames of any sizes and formats) at once: one
+        letterbox launch, one forward of the batch-k engine, one decode launch per head and one batched NMS;
+        `postprocess_batch` waits for the results.  Each frame gets the letterbox and box geometry of its own size."""
         k = len(frames)
         if not 1 <= k <= self.batch:
             raise ValueError(f"expected 1 to {self.batch} frames, got {k}")
-        self.frames_dev = [f if torch.is_tensor(f) else self._upload(b, f) for b, f in enumerate(frames)]
+        self.frames_dev = [self._device(b, f) for b, f in enumerate(frames)]
         geom = self.preprocess_frames(self.frames_dev)
         # a batch-1 input has no image dimension, in this detector and in its batch-1 engine
         inp = self.inp if self.batch == 1 else self.inp[:k] if k > 1 else self.inp[0]
@@ -254,11 +268,21 @@ class YOLODetector(Detector):
         for k in range(1, self.batch + 1):
             self.engine(k)
 
+    def _device(self, b, frame):
+        """Frame b of a call on the device: cuda tensors and device Frames pass through, host frames (HxWx3 ndarrays,
+        host NV12 Frames) go through upload slot b."""
+        if torch.is_tensor(frame) or (isinstance(frame, Frame) and frame.on_device):
+            return frame
+        return self._upload(b, frame)
+
     def _upload(self, b, frame):
-        h, w = frame.shape[:2]
-        if self._uploaders[b] is None or self._uploaders[b].shape != (h, w, 3):
-            self._uploaders[b] = FrameUploader((w, h))
-        return self._uploaders[b].upload(frame)
+        fmt = frame.format if isinstance(frame, Frame) else "BGR"
+        (w, h), host = (frame.size, frame.y) if isinstance(frame, Frame) else ((frame.shape[1], frame.shape[0]), frame)
+        up = self._uploaders[b]
+        if up is None or up.pixel_format != fmt or up.shape != FrameUploader.frame_shape((w, h), fmt):
+            self._uploaders[b] = up = FrameUploader((w, h), pixel_format=fmt)
+        t = up.upload(host)
+        return nv12_frame(t) if fmt == "NV12" else t
 
     def geometry(self, wh):
         """(roi, upscaled_sz, bbox_offset) of frames of size wh = (width, height) in this detector's input."""
@@ -267,14 +291,16 @@ class YOLODetector(Detector):
             self._geometry[wh] = letterbox_geometry(wh, self.input_wh, self.model.LETTERBOX)
         return self._geometry[wh]
 
-    def _upload_geom(self, sizes, frame_ptrs):
-        """Fills one FmFrameGeom row per image, of frame size sizes[b] = (width, height) and device frame pointer
-        frame_ptrs[b] (0 when only the head decode reads the row), and uploads the rows to self._geom in one copy from
-        the pinned block; returns self._geom."""
+    def _upload_geom(self, sizes, frames=None):
+        """Fills one FmFrameGeom row per image, of frame size sizes[b] = (width, height) and device Frame frames[b]
+        (no frame fields when frames is None: only the head decode reads the rows), and uploads the rows to
+        self._geom in one copy from the pinned block; returns self._geom."""
         rows = (_lib.FmFrameGeom * len(sizes))()
-        for r, (w, h), fp in zip(rows, sizes, frame_ptrs):
+        for b, (r, (w, h)) in enumerate(zip(rows, sizes)):
             (rx, ry, rw, rh), up, off = self.geometry((w, h))
-            r.frame, r.w, r.h = fp, w, h
+            if frames is not None:
+                frames[b].fill_geom(r)
+            r.w, r.h = w, h
             r.roi_x, r.roi_y, r.roi_w, r.roi_h = rx, ry, rw, rh
             r.size_w, r.size_h, r.off_x, r.off_y = float(up[0]), float(up[1]), float(off[0]), float(off[1])
         if self._geom_ev is not None:
@@ -287,15 +313,13 @@ class YOLODetector(Detector):
         return self._geom
 
     def preprocess_frames(self, frames_dev):
-        """Letterbox of k frames of any sizes (HxWx3 u8 cuda tensors) into self.inp[:k], one launch.  Uploads
-        their FmFrameGeom table and returns it: the head decode reads it too."""
+        """Letterbox of k frames of any sizes (HxWx3 u8 cuda tensors, or device Frames of either format) into
+        self.inp[:k], one launch.  Uploads their FmFrameGeom table and returns it: the head decode reads it too."""
         k = len(frames_dev)
         if not 1 <= k <= self.batch:
             raise ValueError(f"expected 1 to {self.batch} frames, got {k}")
-        for f in frames_dev:
-            if f.dim() != 3 or f.shape[2] != 3 or f.dtype != torch.uint8 or not f.is_contiguous() or not f.is_cuda:
-                raise ValueError("every frame must be a contiguous HxWx3 uint8 cuda tensor")
-        geom = self._upload_geom([(f.shape[1], f.shape[0]) for f in frames_dev], [f.data_ptr() for f in frames_dev])
+        frames = [f if isinstance(f, Frame) and f.on_device else Frame.bgr(f) for f in frames_dev]
+        geom = self._upload_geom([f.size for f in frames], frames)
         rc = self._lib.fm_letterbox_preproc_geom(ptr(geom), k, self.input_wh[0], self.input_wh[1], ptr(self.inp),
                                                  stream_ptr())
         _lib.check(rc, "fm_letterbox_preproc_geom")
@@ -309,7 +333,7 @@ class YOLODetector(Detector):
         B, k0 = self.batch, self.num_candidates
         k = B if k is None else k
         if geom is None:
-            geom = self._upload_geom([self.size] * k, [0] * k)
+            geom = self._upload_geom([self.size] * k)
         self._k = k
         self._counter.zero_()
         lib = self._lib

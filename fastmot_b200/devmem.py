@@ -103,16 +103,146 @@ class Downlink:
         return out
 
 
-class FrameUploader:
-    """HxWx3 u8 host frame -> device tensor with one async copy.  Page-locked sources (detected with
-    cudaPointerGetAttributes) are copied directly; pageable ones are staged through an internal pinned ring."""
+PIXEL_FORMATS = ("BGR", "NV12")
 
-    def __init__(self, size, depth=2, device="cuda"):
+
+def check_pixel_format(pixel_format):
+    """'BGR' or 'NV12' (any case) -> the upper-case name; anything else raises ValueError."""
+    fmt = str(pixel_format).upper()
+    if fmt not in PIXEL_FORMATS:
+        raise ValueError(f"pixel_format must be one of {PIXEL_FORMATS}, got {pixel_format!r}")
+    return fmt
+
+
+class Frame:
+    """One camera frame as the pre-processing kernels read it: pixel format, size and planes.
+
+    BGR: `y` is an HxWx3 uint8 cuda tensor (tight rows); `uv` is None.
+    NV12 (hardware video decoders): `y` is the H x W luma plane and `uv` the H/2 x W plane of interleaved U, V at half
+    resolution, each with its own row pitch in bytes (`y_pitch`, `uv_pitch` >= W).  A host NV12 frame (`on_device`
+    False) holds its (3H/2, W) ndarray in `y`; FrameUploader turns it into a device frame.  Build NV12 frames with
+    `nv12_frame`; the planes are views of the caller's memory, nothing is copied.
+    """
+    __slots__ = ("format", "w", "h", "y", "uv", "y_pitch", "uv_pitch")
+
+    def __init__(self, format, w, h, y, uv=None, y_pitch=0, uv_pitch=0):
+        self.format, self.w, self.h = format, int(w), int(h)
+        self.y, self.uv, self.y_pitch, self.uv_pitch = y, uv, int(y_pitch), int(uv_pitch)
+
+    @classmethod
+    def bgr(cls, t):
+        """A contiguous HxWx3 uint8 cuda tensor as a Frame."""
+        if not (torch.is_tensor(t) and t.is_cuda and t.dtype == torch.uint8 and t.dim() == 3 and t.shape[2] == 3
+                and t.is_contiguous()):
+            raise ValueError("every BGR frame must be a contiguous HxWx3 uint8 cuda tensor")
+        return cls("BGR", t.shape[1], t.shape[0], t)
+
+    @property
+    def size(self):
+        return (self.w, self.h)
+
+    @property
+    def on_device(self):
+        return torch.is_tensor(self.y)
+
+    def nv12_args(self):
+        """(y, uv, y_pitch, uv_pitch) for the *_nv12 entry points."""
+        return ptr(self.y), ptr(self.uv), self.y_pitch, self.uv_pitch
+
+    def fill_geom(self, row):
+        """Writes the frame fields of one FmFrameGeom row (pointer, size, format)."""
+        from . import _lib
+        row.frame, row.w, row.h = self.y.data_ptr(), self.w, self.h
+        if self.format == "NV12":
+            row.uv, row.pitch, row.uv_pitch, row.format = self.uv.data_ptr(), self.y_pitch, self.uv_pitch, _lib.FM_PIX_NV12
+        else:
+            row.uv, row.pitch, row.uv_pitch, row.format = None, 0, 0, _lib.FM_PIX_BGR
+
+
+def _plane(t, rows, w, what):
+    """Checks one NV12 plane: a 2-D uint8 tensor of `rows` x w with unit column stride and any row stride >= w."""
+    if not torch.is_tensor(t):
+        raise ValueError(f"NV12 {what}: expected a uint8 cuda tensor, got {type(t).__name__}")
+    if t.dtype != torch.uint8 or t.dim() != 2:
+        raise ValueError(f"NV12 {what}: expected a 2-D uint8 tensor, got {t.dtype} of shape {tuple(t.shape)}")
+    if tuple(t.shape) != (rows, w):
+        raise ValueError(f"NV12 {what}: expected shape {(rows, w)}, got {tuple(t.shape)}")
+    if t.stride(1) != 1 or t.stride(0) < w:
+        raise ValueError(f"NV12 {what}: expected stride(1) == 1 and stride(0) >= {w} (the width), got strides "
+                         f"{tuple(t.stride())}")
+
+
+def _even(w, h):
+    if w < 2 or h < 2 or w % 2 or h % 2:
+        raise ValueError(f"NV12 needs an even width and height, got {w}x{h}")
+
+
+def nv12_layout(frame):
+    """Checks the shape, dtype and strides of an NV12 frame in one of the forms `nv12_frame` takes and returns its
+    Frame, without looking at the device its tensors live on."""
+    if isinstance(frame, Frame):
+        if frame.format != "NV12":
+            raise ValueError(f"expected an NV12 frame, got a {frame.format} Frame")
+        return frame
+    if isinstance(frame, (tuple, list)):
+        if len(frame) != 2:
+            raise ValueError(f"NV12 planes: expected a pair (Y (H, W), UV (H/2, W)), got {len(frame)} items")
+        y, uv = frame
+        if not torch.is_tensor(y) or y.dim() != 2:
+            raise ValueError("NV12 Y plane: expected a 2-D uint8 cuda tensor (H, W)")
+        h, w = y.shape
+        _even(w, h)
+        _plane(y, h, w, "Y plane")
+        _plane(uv, h // 2, w, "UV plane")
+        return Frame("NV12", w, h, y, uv, y.stride(0), uv.stride(0))
+    if isinstance(frame, np.ndarray):
+        if frame.dtype != np.uint8 or frame.ndim != 2 or frame.shape[0] % 3:
+            raise ValueError(f"NV12 host frame: expected a (3H/2, W) uint8 ndarray, got {frame.dtype} of shape "
+                             f"{frame.shape}")
+        h, w = frame.shape[0] * 2 // 3, frame.shape[1]
+        _even(w, h)
+        return Frame("NV12", w, h, frame)
+    if torch.is_tensor(frame):
+        if frame.dim() != 2 or frame.shape[0] % 3:
+            raise ValueError(f"NV12 frame: expected a (3H/2, W) uint8 cuda tensor, got shape {tuple(frame.shape)}")
+        h, w = frame.shape[0] * 2 // 3, frame.shape[1]
+        _even(w, h)
+        _plane(frame, 3 * h // 2, w, "frame")
+        return Frame("NV12", w, h, frame[:h], frame[h:], frame.stride(0), frame.stride(0))
+    raise ValueError(f"NV12 frame: expected a (3H/2, W) uint8 ndarray or cuda tensor, or a (Y, UV) pair of cuda "
+                     f"tensors, got {type(frame).__name__}")
+
+
+def nv12_frame(frame):
+    """The Frame of an NV12 frame given as
+      - a host ndarray (3H/2, W) uint8 (Y rows, then UV rows);
+      - a cuda tensor (3H/2, W) uint8 with stride(1) == 1 and any stride(0) >= W (pitched surfaces);
+      - a pair (Y, UV) of cuda tensors (H, W) and (H/2, W), each with its own row stride (decoder surfaces whose UV
+        plane does not follow row H, e.g. 1080p decoded into 1088-row surfaces).
+    A Frame passes through.  Anything else (wrong shape, dtype or device, odd size, row stride below W) raises
+    ValueError naming what was expected."""
+    f = nv12_layout(frame)
+    if f.on_device:
+        if not f.y.is_cuda or not f.uv.is_cuda:
+            raise ValueError(f"NV12 frame: expected cuda tensors, got tensors on {f.y.device} and {f.uv.device} "
+                             "(host frames are (3H/2, W) uint8 ndarrays)")
+        if f.y.device != f.uv.device:
+            raise ValueError(f"NV12 planes on different devices: {f.y.device} and {f.uv.device}")
+    return f
+
+
+class FrameUploader:
+    """Host frame -> device tensor with one async copy: HxWx3 u8 BGR frames, or (pixel_format 'NV12') (3H/2, W) u8
+    NV12 frames, which move half the bytes.  Page-locked sources (detected with cudaPointerGetAttributes) are copied
+    directly; pageable ones are staged through an internal pinned ring."""
+
+    def __init__(self, size, depth=2, device="cuda", pixel_format="BGR"):
         from . import _lib
         self._lib = _lib.load()
-        w, h = size
-        self.shape = (h, w, 3)
-        self.nbytes = h * w * 3
+        self.pixel_format = check_pixel_format(pixel_format)
+        self.shape = self.frame_shape(size, self.pixel_format)
+        self.nbytes = int(np.prod(self.shape))
+        self.bytes_copied = 0              # host-to-device bytes of every copy made so far
         self.dev = [torch.empty(self.shape, dtype=torch.uint8, device=device) for _ in range(depth)]
         self.host = [torch.empty(self.shape, dtype=torch.uint8).pin_memory() for _ in range(depth)]
         self.host_np = [t.numpy() for t in self.host]
@@ -120,9 +250,17 @@ class FrameUploader:
         self.cur = 0
         # read-ahead (GPU-resident ingest, role of the reference's VideoIO frame queue, fastmot/videoio.py:125-142):
         # prefetch(frame) starts the H2D copy of a FUTURE frame on a dedicated upload stream while the current step
-        # computes; upload() of that same frame then only waits for the copy's event.
+        # computes; upload() of that same frame then only waits for the copy's event.  Every prefetched frame keeps its
+        # copy until it is uploaded or its slot is taken again, so prefetch(frame t + 1) issued before upload(frame t)
+        # does not discard frame t's read-ahead.
         self._up_stream = torch.cuda.Stream(device=device)
-        self._prefetched = None            # (key, slot, event)
+        self._prefetched = {}              # key -> (slot, event)
+
+    @staticmethod
+    def frame_shape(size, pixel_format):
+        """Shape of a host frame of size (width, height): (h, w, 3) for BGR, (3h/2, w) for NV12."""
+        w, h = size
+        return (h, w, 3) if pixel_format == "BGR" else (3 * h // 2, w)
 
     @staticmethod
     def _key(frame):
@@ -138,33 +276,56 @@ class FrameUploader:
             src = self.host[k].data_ptr()
         self._lib.fm_memcpy_async(C.c_void_p(self.dev[k].data_ptr()), C.c_void_p(src), self.nbytes,
                                   C.c_void_p(stream.cuda_stream))
+        self.bytes_copied += self.nbytes
         ev = torch.cuda.Event()
         ev.record(stream)
         self.events[k] = ev
         return ev
+
+    def _next_slot(self):
+        """Takes the next ring slot; a read-ahead still parked there is dropped (its frame would be copied again)."""
+        k = self.cur
+        self.cur = (k + 1) % len(self.dev)
+        for key, (slot, _) in list(self._prefetched.items()):
+            if slot == k:
+                del self._prefetched[key]
+        return k
 
     def prefetch(self, frame):
         """Starts the upload of a frame that a later upload() call will ask for (the same ndarray)."""
         frame = np.ascontiguousarray(frame)
         if frame.shape != self.shape or frame.dtype != np.uint8:
             raise ValueError(f"frame must be uint8 {self.shape}, got {frame.dtype} {frame.shape}")
-        k = self.cur
-        self.cur = (k + 1) % len(self.dev)
+        key = self._key(frame)
+        self._prefetched.pop(key, None)          # the array may hold a new frame: copy it again
+        k = self._next_slot()
         # the slot's previous contents may still be read by kernels of the main stream
         self._up_stream.wait_stream(torch.cuda.current_stream())
-        ev = self._copy(frame, k, self._up_stream)
-        self._prefetched = (self._key(frame), k, ev)
+        self._prefetched[key] = (k, self._copy(frame, k, self._up_stream))
 
     def upload(self, frame):
         frame = np.ascontiguousarray(frame)
-        if self._prefetched is not None and self._prefetched[0] == self._key(frame):
-            _, k, ev = self._prefetched
-            self._prefetched = None
+        hit = self._prefetched.pop(self._key(frame), None)
+        if hit is not None:
+            k, ev = hit
             torch.cuda.current_stream().wait_event(ev)
             return self.dev[k]
         if frame.shape != self.shape or frame.dtype != np.uint8:
             raise ValueError(f"frame must be uint8 {self.shape}, got {frame.dtype} {frame.shape}")
-        k = self.cur
-        self.cur = (k + 1) % len(self.dev)
+        k = self._next_slot()
         self._copy(frame, k, torch.cuda.current_stream())
         return self.dev[k]
+
+
+def device_frame(frame, pixel_format, uploader):
+    """A caller's frame as the stages take it: BGR -- the cuda tensor itself, or the uploaded HxWx3 host array; NV12 --
+    the device Frame of any form nv12_frame accepts, host frames uploaded through `uploader` (an NV12 FrameUploader of
+    the frame's size)."""
+    if pixel_format == "BGR":
+        return frame if torch.is_tensor(frame) else uploader.upload(frame)
+    f = nv12_frame(frame)
+    if f.on_device:
+        return f
+    if f.size != (uploader.shape[1], uploader.shape[0] * 2 // 3):
+        raise ValueError(f"NV12 frame of size {f.size}, expected {(uploader.shape[1], uploader.shape[0] * 2 // 3)}")
+    return nv12_frame(uploader.upload(f.y))

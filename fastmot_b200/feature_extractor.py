@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _lib, models
-from .devmem import ptr, stream_ptr, FrameUploader
+from .devmem import ptr, stream_ptr, FrameUploader, Frame, nv12_frame
 from .tracker import DeviceEmbeddings
 
 
@@ -60,7 +60,7 @@ class FeatureExtractor:
         return self.model.METRIC
 
     def extract_async(self, frame, tlbrs):
-        """frame: HxWx3 u8 host array or cuda tensor; tlbrs: (N,4)."""
+        """frame: HxWx3 u8 host array or cuda tensor, or a Frame (an NV12 frame is read in place); tlbrs: (N,4)."""
         tlbrs = np.ascontiguousarray(tlbrs, np.float64).reshape(-1, 4)
         n = len(tlbrs)
         self.last_num_features = n
@@ -70,25 +70,37 @@ class FeatureExtractor:
             return
         if n > self.max_crops:
             raise MemoryError(f"{n} crops > max_crops {self.max_crops}")
-        if torch.is_tensor(frame):
+        if isinstance(frame, Frame) and frame.format == "BGR":
+            frame = frame.y
+        fmt = frame.format if isinstance(frame, Frame) else "BGR"
+        if torch.is_tensor(frame) or (isinstance(frame, Frame) and frame.on_device):
             frame_dev = frame
-            h, w = frame.shape[:2]
         else:
-            h, w = frame.shape[:2]
-            if self._uploader is None or self._uploader.shape != (h, w, 3):
-                self._uploader = FrameUploader((w, h))
-            frame_dev = self._uploader.upload(frame)
+            w, h = frame.size if isinstance(frame, Frame) else (frame.shape[1], frame.shape[0])
+            if self._uploader is None or self._uploader.pixel_format != fmt or \
+                    self._uploader.shape != FrameUploader.frame_shape((w, h), fmt):
+                self._uploader = FrameUploader((w, h), pixel_format=fmt)
+            frame_dev = self._uploader.upload(frame.y if fmt == "NV12" else frame)
+            frame_dev = nv12_frame(frame_dev) if fmt == "NV12" else frame_dev
         eng = self._engine(n)
         self._tlbr_host[:n] = torch.as_tensor(tlbrs)
         self._tlbr_dev[:n].copy_(self._tlbr_host[:n], non_blocking=True)
         c, ih, iw = self.model.INPUT_SHAPE
-        rc = self._lib.fm_roi_resize_norm(ptr(frame_dev), w, h, ptr(self._tlbr_dev), None, n, iw, ih,
-                                          eng.inp_layout, ptr(eng.inp), stream_ptr())
-        _lib.check(rc, "fm_roi_resize_norm")
+        if fmt == "NV12":
+            rc = self._lib.fm_roi_resize_norm_nv12(*frame_dev.nv12_args(), frame_dev.w, frame_dev.h,
+                                                   ptr(self._tlbr_dev), None, n, iw, ih, eng.inp_layout, ptr(eng.inp),
+                                                   stream_ptr())
+            _lib.check(rc, "fm_roi_resize_norm_nv12")
+        else:
+            h, w = frame_dev.shape[:2]
+            rc = self._lib.fm_roi_resize_norm(ptr(frame_dev), w, h, ptr(self._tlbr_dev), None, n, iw, ih,
+                                              eng.inp_layout, ptr(eng.inp), stream_ptr())
+            _lib.check(rc, "fm_roi_resize_norm")
         self._out = eng.forward(n)
 
     def extract_multi_async(self, frames, tlbrs_per_stream):
-        """extract_async over several streams at once: frames[s] (HxWx3 u8 cuda tensors, each of its own size) with
+        """extract_async over several streams at once: frames[s] (HxWx3 u8 cuda tensors or device Frames of either
+        format, each of its own size) with
         its boxes tlbrs_per_stream[s].  All crops are cut in one launch, each clamped to its own frame, and run through
         one OSNet forward (the batch buckets of extract_async hold the sum over streams); `postprocess` then returns
         one slice per stream."""
@@ -106,10 +118,9 @@ class FeatureExtractor:
             raise MemoryError(f"{n} crops > max_crops {self.max_crops}")
         rows = (_lib.FmFrameGeom * len(frames))()
         for r, f in zip(rows, frames):
-            if not torch.is_tensor(f) or not f.is_cuda or f.dtype != torch.uint8 or f.dim() != 3 or f.shape[2] != 3 \
-                    or not f.is_contiguous():
-                raise ValueError("every frame must be a contiguous HxWx3 uint8 cuda tensor")
-            r.frame, r.h, r.w = f.data_ptr(), f.shape[0], f.shape[1]
+            if not (isinstance(f, Frame) and f.on_device):
+                f = Frame.bgr(f)
+            f.fill_geom(r)
         nb = C.sizeof(rows)
         if self._geom_host is None or self._geom_host.numel() < nb:
             if self._geom_ev is not None:

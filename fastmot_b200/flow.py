@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .devmem import ptr, stream_ptr, FrameUploader
+from .devmem import ptr, stream_ptr, FrameUploader, Frame, nv12_frame
 
 LOGGER = logging.getLogger(__name__)
 
@@ -166,6 +166,7 @@ class Flow:
         self._affine_args = (0, size[0], size[1])
         self._h_slots = torch.zeros(max_tracks, dtype=i32).pin_memory()
         self._uploader = FrameUploader(size)
+        self._nv12_uploader = None
         self._side = torch.cuda.Stream()
         self._ev_lk = torch.cuda.Event()
         self._ev_h = torch.cuda.Event()
@@ -271,6 +272,16 @@ class Flow:
 
     # ------------------------------------------------------------------
     def _to_device(self, frame):
+        """BGR frames: the cuda tensor, or the uploaded host array.  A Frame (any format) of this stage's size: the
+        device Frame, host NV12 frames uploaded."""
+        if isinstance(frame, Frame):
+            if frame.size != tuple(self.size):
+                raise ValueError(f"frame of size {frame.size}, the optical-flow stage's is {tuple(self.size)}")
+            if frame.format == "BGR" or frame.on_device:
+                return frame.y if frame.format == "BGR" else frame
+            if self._nv12_uploader is None:
+                self._nv12_uploader = FrameUploader(self.size, pixel_format="NV12")
+            return nv12_frame(self._nv12_uploader.upload(frame.y))
         return frame if torch.is_tensor(frame) else self._uploader.upload(frame)
 
     def _preprocess(self, frame_dev, k):
@@ -278,7 +289,15 @@ class Flow:
         W, H = self.size
         s = stream_ptr()
         lib = self._lib
-        if self._half:
+        if isinstance(frame_dev, Frame):                     # NV12, read in place
+            if self._half:
+                _lib.check(lib.fm_gray_half_nv12(*frame_dev.nv12_args(), W, H, ptr(self.gray[k]),
+                                                 ptr(self.pyr[k][0]), s), "fm_gray_half_nv12")
+            else:
+                sw, sh = self.opt_flow_sz
+                _lib.check(lib.fm_gray_resize_nv12(*frame_dev.nv12_args(), W, H, ptr(self.gray[k]),
+                                                   ptr(self.pyr[k][0]), sw, sh, s), "fm_gray_resize_nv12")
+        elif self._half:
             _lib.check(lib.fm_gray_half(ptr(frame_dev), W, H, ptr(self.gray[k]), ptr(self.pyr[k][0]), s),
                        "fm_gray_half")
         else:
@@ -320,9 +339,14 @@ class Flow:
         runner = self._get_runner()
         if runner is not None:
             main = torch.cuda.current_stream()
-            _lib.check(lib.fm_flow_predict(runner, ptr(frame_dev), self.prev, n, ptr(h_dev), ptr(h_ok_dev),
-                                           C.c_void_p(main.cuda_stream), C.c_void_p(self._side.cuda_stream)),
-                       "fm_flow_predict")
+            if isinstance(frame_dev, Frame):
+                _lib.check(lib.fm_flow_predict_nv12(runner, *frame_dev.nv12_args(), self.prev, n, ptr(h_dev),
+                                                    ptr(h_ok_dev), C.c_void_p(main.cuda_stream),
+                                                    C.c_void_p(self._side.cuda_stream)), "fm_flow_predict_nv12")
+            else:
+                _lib.check(lib.fm_flow_predict(runner, ptr(frame_dev), self.prev, n, ptr(h_dev), ptr(h_ok_dev),
+                                               C.c_void_p(main.cuda_stream), C.c_void_p(self._side.cuda_stream)),
+                           "fm_flow_predict")
             self.prev = cur                      # flow.py:212-213
             self._bg_cache = None
             self._affine_args = (n, W, H)

@@ -16,7 +16,7 @@ import torch
 from .detector import YOLODetector, PublicDetector
 from .feature_extractor import FeatureExtractor
 from .tracker import MultiTracker
-from .devmem import FrameUploader
+from .devmem import FrameUploader, check_pixel_format, device_frame, nv12_frame
 from .utils import Profiler
 
 LOGGER = logging.getLogger(__name__)
@@ -42,8 +42,15 @@ class MOT:
                  draw=False,
                  detections_override=None,
                  embeddings_override=None,
-                 embeddings_tap=None):
+                 embeddings_tap=None,
+                 pixel_format='BGR'):
+        """pixel_format: 'BGR' -- every frame is HxWx3 u8 (host array or cuda tensor); 'NV12' -- every frame is NV12
+        as hardware video decoders emit it, in any form devmem.nv12_frame accepts (host (3H/2, W) array, pitched cuda
+        tensor, or a (Y, UV) pair of cuda planes).  NV12 frames are read in place by the letterbox, crop and KLT
+        kernels; tracks, detections and embeddings are those of the BGR path on cv2.cvtColor(frame,
+        cv2.COLOR_YUV2BGR_NV12)."""
         self.size = size
+        self.pixel_format = check_pixel_format(pixel_format)
         self.detector_type = DetectorType[detector_type.upper()]
         assert detector_frame_skip >= 1
         self.detector_frame_skip = detector_frame_skip
@@ -79,7 +86,7 @@ class MOT:
         self.tracker = MultiTracker(self.size, self.extractors[0].metric, **vars(tracker_cfg),
                                     feat_dim=self.extractors[0].feature_dim)
         self.frame_count = 0
-        self._uploader = FrameUploader(size, depth=3)
+        self._uploader = FrameUploader(size, depth=3, pixel_format=self.pixel_format)
         self._det_stream = torch.cuda.Stream()
         self._main_ready = torch.cuda.Event()
         # ReID crops + OSNet run on their own stream so that the batched Kalman step, its read-back and the host side
@@ -121,12 +128,16 @@ class MOT:
         """Optional read-ahead: starts the host-to-device copy of the NEXT frame (the ndarray a later `step` call will
         receive) on an upload stream, so it overlaps the current step's kernels (role of the reference's VideoIO
         frame queue, fastmot/videoio.py:125-142)."""
-        if not torch.is_tensor(frame):
+        if self.pixel_format == 'NV12':
+            f = nv12_frame(frame)
+            if not f.on_device:
+                self._uploader.prefetch(f.y)
+        elif not torch.is_tensor(frame):
             self._uploader.prefetch(frame)
 
     def step(self, frame):
         """mot.py:125-168"""
-        frame_dev = frame if torch.is_tensor(frame) else self._uploader.upload(frame)
+        frame_dev = device_frame(frame, self.pixel_format, self._uploader)
         detections = []
         if self.frame_count == 0:
             self._detect_async(frame_dev)

@@ -21,7 +21,7 @@ import torch
 from .detector import YOLODetector
 from .feature_extractor import FeatureExtractor
 from .tracker import MultiTracker
-from .devmem import FrameUploader
+from .devmem import FrameUploader, check_pixel_format, device_frame, nv12_frame
 from .mot import DetectorType
 from .utils import Profiler
 
@@ -57,8 +57,10 @@ class MultiCameraMOT:
                  visualizer_cfg=None,
                  draw=False,
                  detections_override=None,
-                 embeddings_override=None):
-        """sizes: one (width, height) per camera.  The keyword arguments are MOT's, so the reference's `mot_cfg`
+                 embeddings_override=None,
+                 pixel_format='BGR'):
+        """sizes: one (width, height) per camera.  pixel_format ('BGR' or 'NV12', as in MOT) applies to every
+        camera of the group.  The keyword arguments are MOT's, so the reference's `mot_cfg`
         (cfg/mot.json) passes unchanged; ssd_detector_cfg, public_detector_cfg and visualizer_cfg are accepted and
         unused, since only the YOLO detector runs several cameras.  detections_override(camera, frame_id) and
         embeddings_override(camera, frame_id, detections) replace the networks' OUTPUT after both ran, as MOT's hooks
@@ -71,6 +73,7 @@ class MultiCameraMOT:
                 raise ValueError(f"every camera size must be (width, height), got {wh!r}")
             self.sizes.append(tuple(int(v) for v in wh))
         self.num_cameras = N = len(self.sizes)
+        self.pixel_format = check_pixel_format(pixel_format)
         self.detector_type = DetectorType[detector_type.upper()]
         if self.detector_type != DetectorType.YOLO:
             raise NotImplementedError(f"detector_type {detector_type!r}: several cameras are tracked with the batched "
@@ -103,7 +106,7 @@ class MultiCameraMOT:
         self.trackers = [MultiTracker(wh, self.extractors[0].metric, **vars(tracker_cfg),
                                       feat_dim=self.extractors[0].feature_dim) for wh in self.sizes]
         self.frame_counts = [0] * N
-        self._uploaders = [FrameUploader(wh, depth=3) for wh in self.sizes]
+        self._uploaders = [FrameUploader(wh, depth=3, pixel_format=self.pixel_format) for wh in self.sizes]
         self._det_stream = torch.cuda.Stream()
         self._main_ready = torch.cuda.Event()
         self._reid_stream = torch.cuda.Stream()
@@ -130,14 +133,25 @@ class MultiCameraMOT:
         """Starts the uploads of the frames a later `step` call will receive (host arrays only; None is skipped)."""
         self._check_frames(frames)
         for up, f in zip(self._uploaders, frames):
-            if f is not None and not torch.is_tensor(f):
+            if f is None:
+                continue
+            if self.pixel_format == 'NV12':
+                f = nv12_frame(f)
+                if not f.on_device:
+                    up.prefetch(f.y)
+            elif not torch.is_tensor(f):
                 up.prefetch(f)
 
     def _check_frames(self, frames):
         if len(frames) != self.num_cameras:
             raise ValueError(f"expected {self.num_cameras} frames, got {len(frames)}")
         for s, (f, (w, h)) in enumerate(zip(frames, self.sizes)):
-            if f is not None and tuple(f.shape) != (h, w, 3):
+            if f is None:
+                continue
+            if self.pixel_format == 'NV12':
+                if nv12_frame(f).size != (w, h):
+                    raise ValueError(f"camera {s}: NV12 frame of size {nv12_frame(f).size}, expected {(w, h)}")
+            elif tuple(f.shape) != (h, w, 3):
                 raise ValueError(f"camera {s}: frame of shape {tuple(f.shape)}, expected {(h, w, 3)}")
 
     def _detect_async(self, frames_dev):
@@ -153,10 +167,10 @@ class MultiCameraMOT:
         return dict(zip(cams, dets))
 
     def step(self, frames):
-        """One step of the group: frames[s] is camera s's next HxWx3 u8 frame (host array or cuda tensor), or None
-        when camera s has no frame on this step."""
+        """One step of the group: frames[s] is camera s's next frame in the group's pixel format (HxWx3 u8 host array
+        or cuda tensor; NV12 in any form MOT takes), or None when camera s has no frame on this step."""
         self._check_frames(frames)
-        frames_dev = [None if f is None else f if torch.is_tensor(f) else up.upload(f)
+        frames_dev = [None if f is None else device_frame(f, self.pixel_format, up)
                       for f, up in zip(frames, self._uploaders)]
         init, detect, track = plan_step(self.frame_counts, [f is not None for f in frames], self.detector_frame_skip)
         cams = sorted(init + detect)                 # the detector batch, in camera order

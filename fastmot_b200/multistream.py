@@ -24,8 +24,10 @@ class MultiStreamMOT(MultiCameraMOT):
                  visualizer_cfg=None,
                  draw=False,
                  detections_override=None,
-                 embeddings_override=None):
-        """size: (width, height) shared by every stream.  The keyword arguments are MOT's, so the reference's
+                 embeddings_override=None,
+                 pixel_format='BGR'):
+        """size: (width, height) shared by every stream; pixel_format ('BGR' or 'NV12', as in MOT) applies to every
+        stream.  The keyword arguments are MOT's, so the reference's
         `mot_cfg` (cfg/mot.json) passes unchanged; ssd_detector_cfg, public_detector_cfg and visualizer_cfg are
         accepted and unused, since only the YOLO detector runs several streams.  detections_override(stream,
         frame_id) and embeddings_override(stream, frame_id, detections) replace the networks' OUTPUT after both ran,
@@ -42,7 +44,8 @@ class MultiStreamMOT(MultiCameraMOT):
                          ssd_detector_cfg=ssd_detector_cfg, yolo_detector_cfg=yolo_detector_cfg,
                          public_detector_cfg=public_detector_cfg, feature_extractor_cfgs=feature_extractor_cfgs,
                          tracker_cfg=tracker_cfg, visualizer_cfg=visualizer_cfg, draw=draw,
-                         detections_override=detections_override, embeddings_override=embeddings_override)
+                         detections_override=detections_override, embeddings_override=embeddings_override,
+                         pixel_format=pixel_format)
 
     @property
     def frame_count(self):
@@ -50,7 +53,8 @@ class MultiStreamMOT(MultiCameraMOT):
         return self.frame_counts[0]
 
     def step(self, frames):
-        """One step of every stream: frames[s] is stream s's next HxWx3 u8 frame (host array or cuda tensor)."""
+        """One step of every stream: frames[s] is stream s's next frame (HxWx3 u8 host array or cuda tensor; NV12 in
+        any form MOT takes when pixel_format is 'NV12')."""
         if any(f is None for f in frames):
             raise ValueError("every stream delivers a frame on every step; cameras that skip steps need "
                              "MultiCameraMOT")
