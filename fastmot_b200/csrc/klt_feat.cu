@@ -302,69 +302,37 @@ __device__ __forceinline__ unsigned desc_key(float v) {
     return (u & 0x80000000u) ? u : ~(u | 0x80000000u);
 }
 
-// threshold + 3x3 local maximum + sort (value desc, address desc) + greedy min-distance + ellipse filter.
-// kGeneral = false: the default settings (response > 0, at most 1024 corners kept in shared memory).  kGeneral = true:
-// any response sign (THRESH_TOZERO is applied to the neighbours before the local-maximum test, as OpenCV's dilate
-// sees them), maxCorners <= 0 means no limit, and the accepted corners go to acc_list (two ints per corner, in the
-// gradient planes of this track's scratch, free once the response is final).
-#define GFTT_MAX_CAND 4096
+// Candidate test of the selection: interior pixel of the crop, response above the quality threshold, seen by track k,
+// 3x3 local maximum.  On success `key` is the sort key: ascending u64 == value desc, then crop pixel index desc
+// (OpenCV's greaterThanPtr order).
 template <bool kGeneral>
-__global__ void __launch_bounds__(256) gftt_select_kernel(const int* __restrict__ owner, int w, int h,
-                                                           const double* __restrict__ tlbr_pool,
-                                                           FmTrackJob* __restrict__ jobs, int n_trk,
-                                                           const float* __restrict__ scratch, double quality,
-                                                           int max_corners, float* __restrict__ kp_pool,
-                                                           int* __restrict__ kp_count, int max_kp,
-                                                           int* __restrict__ status, float* __restrict__ acc_scratch) {
-    __shared__ unsigned long long s_key[GFTT_MAX_CAND];
-    __shared__ unsigned char s_dead[GFTT_MAX_CAND];
-    __shared__ int s_n, s_nacc, s_cur;
-    __shared__ short s_accx[kGeneral ? 1 : 1024], s_accy[kGeneral ? 1 : 1024];
-    const int k = blockIdx.x;
-    if (k >= n_trk) return;
-    const FmTrackJob job = jobs[k];
-    if (job.redetect == 2 && threadIdx.x == 0) status[0] = 2;
-    if (job.redetect != 1) return;
-    const int cw = job.cw, ch = job.ch, tid = threadIdx.x;
-    const float* eig = scratch + job.scratch_off;
-    int* acc_list = kGeneral ? (int*)(acc_scratch + job.scratch_off + cw * ch) : nullptr;
-    const float thr = (float)((double)job.eig_max * quality);
-    if (tid == 0) { s_n = 0; s_nacc = 0; }
-    __syncthreads();
-    for (int i = tid; i < cw * ch; i += blockDim.x) {
-        const int y = i / cw, x = i - y * cw;
-        if (y < 1 || x < 1 || y >= ch - 1 || x >= cw - 1) continue;
-        const float v = eig[i];
-        if (!(v > thr)) continue;  // THRESH_TOZERO then `val != 0`
-        if (kGeneral && v == 0.f) continue;
-        if (owner[(size_t)(job.y0 + y) * w + job.x0 + x] != k) continue;
-        bool ismax = true;
+__device__ __forceinline__ bool gftt_candidate(const float* __restrict__ eig, const int* __restrict__ owner, int w,
+                                               const FmTrackJob& job, int k, float thr, int i,
+                                               unsigned long long& key) {
+    const int cw = job.cw, ch = job.ch;
+    const int y = i / cw, x = i - y * cw;
+    if (y < 1 || x < 1 || y >= ch - 1 || x >= cw - 1) return false;
+    const float v = eig[i];
+    if (!(v > thr)) return false;  // THRESH_TOZERO then `val != 0`
+    if (kGeneral && v == 0.f) return false;
+    if (owner[(size_t)(job.y0 + y) * w + job.x0 + x] != k) return false;
+    bool ismax = true;
 #pragma unroll
-        for (int dy = -1; dy <= 1; ++dy)
+    for (int dy = -1; dy <= 1; ++dy)
 #pragma unroll
-            for (int dx = -1; dx <= 1; ++dx) {
-                float nb = eig[(y + dy) * cw + (x + dx)];
-                if (kGeneral && !(nb > thr)) nb = 0.f;
-                ismax = ismax && (v >= nb);
-            }
-        if (!ismax) continue;
-        const int pos = atomicAdd(&s_n, 1);
-        if (pos < GFTT_MAX_CAND) {
-            // ascending u64 sort == value desc (v > 0), then pixel index desc
-            const unsigned vk = kGeneral ? desc_key(v) : ~__float_as_uint(v);
-            s_key[pos] = ((unsigned long long)vk << 32) | (unsigned)(0x7fffffff - i);
+        for (int dx = -1; dx <= 1; ++dx) {
+            float nb = eig[(y + dy) * cw + (x + dx)];
+            if (kGeneral && !(nb > thr)) nb = 0.f;
+            ismax = ismax && (v >= nb);
         }
-    }
-    __syncthreads();
-    int n = s_n;
-    if (n > GFTT_MAX_CAND) {
-        if (tid == 0) status[0] = 3;  // candidate overflow, surfaced to the host
-        n = GFTT_MAX_CAND;
-    }
-    int np2 = 1;
-    while (np2 < n) np2 <<= 1;
-    for (int i = n + tid; i < np2; i += blockDim.x) s_key[i] = ~0ull;
-    __syncthreads();
+    if (!ismax) return false;
+    // value desc (the default setting's responses are > 0, so the inverted bits order them), then pixel index desc
+    const unsigned vk = kGeneral ? desc_key(v) : ~__float_as_uint(v);
+    key = ((unsigned long long)vk << 32) | (unsigned)(0x7fffffff - i);
+    return true;
+}
+
+__device__ __forceinline__ void bitonic_sort_smem(unsigned long long* s_key, int np2, int tid) {
     for (int kk = 2; kk <= np2; kk <<= 1)
         for (int j = kk >> 1; j > 0; j >>= 1) {
             for (int t = tid; t < (np2 >> 1); t += blockDim.x) {
@@ -375,37 +343,245 @@ __global__ void __launch_bounds__(256) gftt_select_kernel(const int* __restrict_
             }
             __syncthreads();
         }
-    for (int i = tid; i < n; i += blockDim.x) s_dead[i] = 0;
+}
+
+// One pass of the block-wide merge sort: the sorted runs [2r*q, 2r*q + r) and [2r*q + r, 2r*(q+1)) of src are merged
+// into dst.  Each thread writes GFTT_MERGE_ITEMS consecutive outputs of one pair (the count divides 2r) after a
+// merge-path search for how many of them come from the first run.  The keys are unique and never ~0.
+#define GFTT_MERGE_ITEMS 32
+__device__ __forceinline__ void merge_pass(const unsigned long long* src, unsigned long long* dst, int n, int run,
+                                           int tid) {
+    for (int o = tid * GFTT_MERGE_ITEMS; o < n; o += blockDim.x * GFTT_MERGE_ITEMS) {
+        const int base = o - o % (2 * run);
+        const int na = min(run, n - base);
+        const int nb = min(run, n - base - na);
+        const unsigned long long* A = src + base;
+        const unsigned long long* B = A + na;
+        const int d = o - base;
+        int lo = d > nb ? d - nb : 0, hi = d < na ? d : na;
+        while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (A[mid] < B[d - 1 - mid]) lo = mid + 1;
+            else hi = mid;
+        }
+        int ai = lo, bi = d - lo;
+        unsigned long long ka = ai < na ? A[ai] : ~0ull, kb = bi < nb ? B[bi] : ~0ull;
+        const int end = d + GFTT_MERGE_ITEMS < na + nb ? d + GFTT_MERGE_ITEMS : na + nb;
+        for (int q = d; q < end; ++q) {
+            if (ka < kb) { dst[base + q] = ka; ++ai; ka = ai < na ? A[ai] : ~0ull; }
+            else { dst[base + q] = kb; ++bi; kb = bi < nb ? B[bi] : ~0ull; }
+        }
+    }
+}
+
+// threshold + 3x3 local maximum + sort (value desc, address desc) + greedy min-distance + ellipse filter.
+// kGeneral = false: the default settings (response > 0, at most 1024 corners kept in shared memory).  kGeneral = true:
+// any response sign (THRESH_TOZERO is applied to the neighbours before the local-maximum test, as OpenCV's dilate
+// sees them), maxCorners <= 0 means no limit, and the accepted corners go to acc_list (two ints per corner, in the
+// gradient planes of this track's scratch, free once the response is final).
+//
+// A box of at most GFTT_MAX_CAND candidates sorts its keys in shared memory and runs the greedy loop there (one barrier
+// pair per accepted corner, each scanning the remaining candidates).  A box with more claims its candidate storage from
+// `work` through the per-frame scratch counter (status 2 when it does not fit) and runs the same selection in global
+// memory: keys re-collected, sorted as GFTT_MAX_CAND-key shared-memory chunks merged pass by pass, then the greedy loop
+// over chunks of 256 sorted candidates against a grid of minDistance cells holding the accepted corners (OpenCV's own
+// structure): every thread tests one candidate against the 3x3 cells around it, then warp 0 settles the chunk's
+// survivors in order.  Both paths accept exactly the corners of the sequential greedy.  Kept corners beyond max_kp
+// set status 4.
+#define GFTT_MAX_CAND 4096
+constexpr int kSelectThreads = 256;
+template <bool kGeneral>
+__global__ void __launch_bounds__(kSelectThreads) gftt_select_kernel(const int* __restrict__ owner, int w, int h,
+                                                                      const double* __restrict__ tlbr_pool,
+                                                                      FmTrackJob* __restrict__ jobs, int n_trk,
+                                                                      const float* __restrict__ scratch,
+                                                                      double quality, int max_corners,
+                                                                      float* __restrict__ kp_pool,
+                                                                      int* __restrict__ kp_count, int max_kp,
+                                                                      int* __restrict__ status,
+                                                                      float* __restrict__ work,
+                                                                      int* __restrict__ scratch_counter,
+                                                                      int scratch_cap) {
+    __shared__ unsigned long long s_key[GFTT_MAX_CAND];
+    __shared__ unsigned char s_dead[GFTT_MAX_CAND];
+    __shared__ int s_n, s_nacc, s_cur, s_off;
+    __shared__ short s_accx[kGeneral ? 1 : 1024], s_accy[kGeneral ? 1 : 1024];
+    __shared__ int s_cidx[kSelectThreads];
+    const int k = blockIdx.x;
+    if (k >= n_trk) return;
+    const FmTrackJob job = jobs[k];
+    if (job.redetect == 2 && threadIdx.x == 0) status[0] = 2;
+    if (job.redetect != 1) return;
+    const int cw = job.cw, ch = job.ch, tid = threadIdx.x;
+    const float* eig = scratch + job.scratch_off;
+    int* acc_list = kGeneral ? (int*)(work + job.scratch_off + cw * ch) : nullptr;
+    const float thr = (float)((double)job.eig_max * quality);
+    if (tid == 0) { s_n = 0; s_nacc = 0; }
     __syncthreads();
-    // greedy min-distance: one barrier pair per ACCEPTED corner
+    for (int i = tid; i < cw * ch; i += blockDim.x) {
+        unsigned long long key;
+        if (!gftt_candidate<kGeneral>(eig, owner, w, job, k, thr, i, key)) continue;
+        const int pos = atomicAdd(&s_n, 1);
+        if (pos < GFTT_MAX_CAND) s_key[pos] = key;
+    }
+    __syncthreads();
+    const int n = s_n;
     const int md2 = job.min_dist * job.min_dist;
-    int cur = 0;
     const int cap = kGeneral ? (max_corners > 0 ? max_corners : INT_MAX) : min(max_corners, 1024);
-    while (true) {
+    if (n <= GFTT_MAX_CAND) {
+        int np2 = 1;
+        while (np2 < n) np2 <<= 1;
+        for (int i = n + tid; i < np2; i += blockDim.x) s_key[i] = ~0ull;
+        __syncthreads();
+        bitonic_sort_smem(s_key, np2, tid);
+        for (int i = tid; i < n; i += blockDim.x) s_dead[i] = 0;
+        __syncthreads();
+        // greedy min-distance: one barrier pair per ACCEPTED corner
+        int cur = 0;
+        while (true) {
+            if (tid == 0) {
+                int c = cur;
+                while (c < n && s_dead[c]) ++c;
+                s_cur = (s_nacc < cap) ? c : n;
+            }
+            __syncthreads();
+            cur = s_cur;
+            if (cur >= n) break;
+            const int idx = 0x7fffffff - (int)(s_key[cur] & 0xffffffffu);
+            const int cy = idx / cw, cx = idx - cy * cw;
+            if (tid == 0) {
+                if (kGeneral) { acc_list[2 * s_nacc] = cx; acc_list[2 * s_nacc + 1] = cy; }
+                else { s_accx[s_nacc] = cx; s_accy[s_nacc] = cy; }
+                s_nacc = s_nacc + 1;
+            }
+            for (int j = cur + 1 + tid; j < n; j += blockDim.x) {
+                if (s_dead[j]) continue;
+                const int ji = 0x7fffffff - (int)(s_key[j] & 0xffffffffu);
+                const int jy = ji / cw, jx = ji - jy * cw;
+                const int dx = jx - cx, dy = jy - cy;
+                if (dx * dx + dy * dy < md2) s_dead[j] = 1;
+            }
+            ++cur;
+            __syncthreads();
+        }
+    } else {
+        // ---- global-memory path.  Layout from an 8-byte aligned start: keys[n], sort buffer[n] (u64), accepted-corner
+        // nodes {crop index, next} [min(n, cap)] (int2), grid cell heads [gw * gh] (int, -1 = empty).
+        const int md = job.min_dist;
+        const int gw = (cw + md - 1) / md, gh = (ch + md - 1) / md;
+        // the default setting's cap (at most 1024) is below n; min(n, cap) there would chain onto cap's own min,
+        // which ptxas fuses into a VIMNMX3 (DESIGN section 4)
+        const int n_node = !kGeneral ? cap : (n < cap ? n : cap);
+        const long long need = 4ll * n + 2ll * n_node + (long long)gw * gh + 1;
         if (tid == 0) {
-            int c = cur;
-            while (c < n && s_dead[c]) ++c;
-            s_cur = (s_nacc < cap) ? c : n;
+            int off = -1;
+            if (need <= (long long)scratch_cap) {
+                const int o = atomicAdd(scratch_counter, (int)need);
+                if (o >= 0 && (long long)o + need <= (long long)scratch_cap) off = o;
+            }
+            if (off < 0) status[0] = 2;  // raise scratch_floats
+            s_off = off;
+            s_cur = 0;
         }
         __syncthreads();
-        cur = s_cur;
-        if (cur >= n) break;
-        const int idx = 0x7fffffff - (int)(s_key[cur] & 0xffffffffu);
-        const int cy = idx / cw, cx = idx - cy * cw;
-        if (tid == 0) {
-            if (kGeneral) { acc_list[2 * s_nacc] = cx; acc_list[2 * s_nacc + 1] = cy; }
-            else { s_accx[s_nacc] = cx; s_accy[s_nacc] = cy; }
-            s_nacc = s_nacc + 1;
-        }
-        for (int j = cur + 1 + tid; j < n; j += blockDim.x) {
-            if (s_dead[j]) continue;
-            const int ji = 0x7fffffff - (int)(s_key[j] & 0xffffffffu);
-            const int jy = ji / cw, jx = ji - jy * cw;
-            const int dx = jx - cx, dy = jy - cy;
-            if (dx * dx + dy * dy < md2) s_dead[j] = 1;
-        }
-        ++cur;
+        if (s_off < 0) return;
+        unsigned long long* keys = (unsigned long long*)(work + ((s_off + 1) & ~1));
+        unsigned long long* tmp = keys + n;
+        int2* nodes = (int2*)(tmp + n);
+        int* heads = (int*)(nodes + n_node);
+        const int lane = tid & 31, wid = tid >> 5;
+        for (int i = tid; i < gw * gh; i += blockDim.x) heads[i] = -1;
         __syncthreads();
+        // re-collect the keys, one shared-memory atomic per warp
+        for (int base = 0; base < cw * ch; base += blockDim.x) {
+            const int i = base + tid;
+            unsigned long long key = 0;
+            const bool c = i < cw * ch && gftt_candidate<kGeneral>(eig, owner, w, job, k, thr, i, key);
+            const unsigned bal = __ballot_sync(0xffffffffu, c);
+            int wpos = 0;
+            if (lane == 0 && bal) wpos = atomicAdd(&s_cur, __popc(bal));
+            wpos = __shfl_sync(0xffffffffu, wpos, 0);
+            if (c) keys[wpos + __popc(bal & ((1u << lane) - 1u))] = key;
+        }
+        __syncthreads();
+        // sort: shared-memory bitonic chunks of GFTT_MAX_CAND keys, then merge passes (keys <-> tmp)
+        for (int c0 = 0; c0 < n; c0 += GFTT_MAX_CAND) {
+            for (int i = tid; i < GFTT_MAX_CAND; i += blockDim.x) s_key[i] = c0 + i < n ? keys[c0 + i] : ~0ull;
+            __syncthreads();
+            bitonic_sort_smem(s_key, GFTT_MAX_CAND, tid);
+            for (int i = tid; i < GFTT_MAX_CAND && c0 + i < n; i += blockDim.x) keys[c0 + i] = s_key[i];
+            __syncthreads();
+        }
+        unsigned long long* src = keys;
+        unsigned long long* dst = tmp;
+        for (int run = GFTT_MAX_CAND; run < n; run <<= 1) {
+            merge_pass(src, dst, n, run, tid);
+            __syncthreads();
+            unsigned long long* t = src; src = dst; dst = t;
+        }
+        // greedy min-distance over chunks of kSelectThreads sorted candidates
+        for (int c0 = 0; c0 < n; c0 += kSelectThreads) {
+            const int j = c0 + tid;
+            int idx = 0;
+            bool alive = false;
+            if (j < n) {
+                idx = 0x7fffffff - (int)(src[j] & 0xffffffffu);
+                const int cy = idx / cw, cx = idx - cy * cw, gx = cx / md, gy = cy / md;
+                alive = true;
+                for (int yy = gy - 1; yy <= gy + 1; ++yy) {
+                    if (yy < 0 || yy >= gh) continue;
+                    for (int xx = gx - 1; xx <= gx + 1; ++xx) {
+                        if (xx < 0 || xx >= gw) continue;
+                        for (int a = heads[yy * gw + xx]; a >= 0 && alive; ) {
+                            const int2 nd = nodes[a];
+                            const int ay = nd.x / cw, ax = nd.x - ay * cw;
+                            const int dx = ax - cx, dy = ay - cy;
+                            alive = dx * dx + dy * dy >= md2;
+                            a = nd.y;
+                        }
+                    }
+                }
+            }
+            s_cidx[tid] = idx;
+            s_dead[tid] = alive;
+            __syncthreads();
+            if (wid == 0) {
+                // lane l holds candidates l, l + 32, ... of the chunk; live[g] has a bit per candidate still to settle
+                int px[kSelectThreads / 32], py[kSelectThreads / 32];
+                unsigned live[kSelectThreads / 32];
+#pragma unroll
+                for (int g = 0; g < kSelectThreads / 32; ++g) {
+                    const int id = s_cidx[32 * g + lane];
+                    py[g] = id / cw; px[g] = id - py[g] * cw;
+                    live[g] = __ballot_sync(0xffffffffu, s_dead[32 * g + lane] != 0);
+                }
+                int nacc = s_nacc;
+#pragma unroll
+                for (int g = 0; g < kSelectThreads / 32; ++g) {
+                    while (live[g] != 0u && nacc < cap) {
+                        // the first live candidate is accepted; it kills every later one closer than minDistance
+                        const int f = __ffs(live[g]) - 1;
+                        const int fx = __shfl_sync(0xffffffffu, px[g], f), fy = __shfl_sync(0xffffffffu, py[g], f);
+                        if (lane == 0) {
+                            if (kGeneral) { acc_list[2 * nacc] = fx; acc_list[2 * nacc + 1] = fy; }
+                            else { s_accx[nacc] = fx; s_accy[nacc] = fy; }
+                            const int cell = (fy / md) * gw + fx / md;
+                            nodes[nacc] = make_int2(fy * cw + fx, heads[cell]);
+                            heads[cell] = nacc;
+                        }
+                        ++nacc;
+#pragma unroll
+                        for (int g2 = g; g2 < kSelectThreads / 32; ++g2) {
+                            const int dx = px[g2] - fx, dy = py[g2] - fy;
+                            live[g2] &= ~__ballot_sync(0xffffffffu, dx * dx + dy * dy < md2);
+                        }
+                    }
+                }
+                if (lane == 0) s_nacc = nacc;
+            }
+            __syncthreads();
+            if (s_nacc >= cap) break;
+        }
     }
     __syncthreads();
     // _ellipse_filter (flow.py:298-306): pts + offset (f32), inside the ellipse inscribed in the FULL box
@@ -415,11 +591,14 @@ __global__ void __launch_bounds__(256) gftt_select_kernel(const int* __restrict_
         const double ax = (t[2] - t[0] + 1) * 0.5, ay = (t[3] - t[1] + 1) * 0.5;
         float* kp = kp_pool + (size_t)job.slot * max_kp * 2;
         int m = 0;
-        for (int i = 0; i < s_nacc && m < max_kp; ++i) {
+        for (int i = 0; i < s_nacc; ++i) {
             const int ax_i = kGeneral ? acc_list[2 * i] : s_accx[i], ay_i = kGeneral ? acc_list[2 * i + 1] : s_accy[i];
             const float px = (float)ax_i + (float)job.x0, py = (float)ay_i + (float)job.y0;
             const double ux = ((double)px - ccx) / ax, uy = ((double)py - ccy) / ay;
-            if (ux * ux + uy * uy <= 1.0) { kp[2 * m] = px; kp[2 * m + 1] = py; ++m; }
+            if (ux * ux + uy * uy <= 1.0) {
+                if (m == max_kp) { status[0] = 4; break; }  // more kept corners than keypoint rows
+                kp[2 * m] = px; kp[2 * m + 1] = py; ++m;
+            }
         }
         kp_count[job.slot] = m;
     }
@@ -611,8 +790,9 @@ extern "C" int fm_flow_keypoints(const unsigned char* prev_gray, int w, int h, c
         kp_prepare_kernel<<<n_trk, 256, 0, s>>>(tlbr_pool, slots, n_trk, w, h, owner, kp_pool, kp_count, max_kp,
                                                 feat_density, feat_dist_factor, jobs, scratch_counter, scratch_cap, 1);
         gftt_eig_kernel<<<n_trk, 256, 0, s>>>(prev_gray, w, h, owner, jobs, n_trk, scratch);
-        gftt_select_kernel<false><<<n_trk, 256, 0, s>>>(owner, w, h, tlbr_pool, jobs, n_trk, scratch, quality,
-                                                        max_corners, kp_pool, kp_count, max_kp, status, nullptr);
+        gftt_select_kernel<false><<<n_trk, kSelectThreads, 0, s>>>(owner, w, h, tlbr_pool, jobs, n_trk, scratch,
+                                                                   quality, max_corners, kp_pool, kp_count, max_kp,
+                                                                   status, scratch, scratch_counter, scratch_cap);
     }
     FM_CHECK_LAUNCH("fm_flow_keypoints");
     return FM_OK;
@@ -644,8 +824,9 @@ extern "C" int fm_flow_keypoints_cfg(const unsigned char* prev_gray, int w, int 
                                                 feat_density, feat_dist_factor, jobs, scratch_counter, scratch_cap, 4);
         gftt_response_kernel<<<n_trk, 256, 0, s>>>(prev_gray, w, h, owner, jobs, n_trk, scratch, block_size,
                                                    gradient_size, use_harris, (float)harris_k);
-        gftt_select_kernel<true><<<n_trk, 256, 0, s>>>(owner, w, h, tlbr_pool, jobs, n_trk, scratch, quality,
-                                                       max_corners, kp_pool, kp_count, max_kp, status, scratch);
+        gftt_select_kernel<true><<<n_trk, kSelectThreads, 0, s>>>(owner, w, h, tlbr_pool, jobs, n_trk, scratch,
+                                                                  quality, max_corners, kp_pool, kp_count, max_kp,
+                                                                  status, scratch, scratch_counter, scratch_cap);
     }
     FM_CHECK_LAUNCH("fm_flow_keypoints_cfg");
     return FM_OK;

@@ -20,7 +20,9 @@ from .devmem import ptr, stream_ptr, FrameUploader, Frame, nv12_frame
 
 LOGGER = logging.getLogger(__name__)
 
-# candidate corners one box may hold in the selection kernel (csrc/klt_feat.cu GFTT_MAX_CAND); more raise at run time
+# candidate corners the selection kernel sorts in shared memory (csrc/klt_feat.cu GFTT_MAX_CAND); a box with more
+# selects them in global memory from scratch_floats.  Also the keypoint rows a track has when maxCorners is <= 0 or
+# above 4096: more kept corners raise at run time
 GFTT_MAX_CAND = 4096
 # keyword arguments of cv2.goodFeaturesToTrack that obj_feat_params may set (minDistance and mask come from the track)
 _GFTT_KEYS = {"maxCorners", "qualityLevel", "blockSize", "useHarrisDetector", "k", "gradientSize"}
@@ -440,8 +442,15 @@ class Flow:
     def check_flags(self, hf):
         """hf: the 32 status ints copied back.  Raises on overflow; returns True when the rounds converged."""
         n = self._affine_args[0]
+        if hf[1] == 2:
+            raise MemoryError("Flow scratch overflow (code 2): the corner re-detection of this frame's boxes needs more "
+                              f"than scratch_floats={self.scratch_cap} floats; raise scratch_floats")
+        if hf[1] == 4:
+            raise MemoryError(f"Flow keypoint overflow (code 4): a track kept more corners than its {self.max_kp} "
+                              f"keypoint rows (maxCorners={self.obj_feat_params['maxCorners']}; at most "
+                              f"{GFTT_MAX_CAND} rows per track); set maxCorners between 1 and {GFTT_MAX_CAND}")
         if hf[1] != 0:
-            raise MemoryError(f"Flow scratch/candidate overflow (code {int(hf[1])}); raise scratch_floats")
+            raise MemoryError(f"Flow keypoint status code {int(hf[1])}")
         return n == 0 or hf[8 + ((self.rounds_last - 1) & 15)] == 0 or self.rounds_last >= 2 * max(n, 1) + 2
 
     def finish_rounds(self, rounds=None):

@@ -373,8 +373,10 @@ int fm_bg_small(const unsigned char* gray, const int* owner, int w, int h, unsig
 /* flow.py:156-184 for all active tracks (slots[] in nearest-first order, boxes from tlbr_pool): occlusion/owner
  * map, keypoint filtering (_rect_filter), Shi-Tomasi re-detection (cv2.goodFeaturesToTrack, blockSize 3, gradient
  * aperture 3, 0 < max_corners <= 1024) where len(kp) < feat_density * area, ellipse filter.  Keypoints live in
- * kp_pool[cap][max_kp][2] / kp_count[cap].  scratch: scratch_cap floats for the eigenvalue maps; status[0] != 0
- * reports scratch (2) or candidate (3, more than 4096 local maxima in one box) overflow. */
+ * kp_pool[cap][max_kp][2] / kp_count[cap].  scratch: scratch_cap floats for the eigenvalue maps and, for a box with
+ * more than 4096 candidate corners (local maxima above the quality threshold), 4 floats per candidate, 2 per accepted
+ * corner and one per minDistance cell of the box; status[0] != 0 reports scratch (2) or keypoint (4, more kept corners in one box than
+ * max_kp) overflow. */
 int fm_flow_keypoints(const unsigned char* prev_gray, int w, int h, const double* tlbr_pool, const int* slots,
                       int n_trk, int* owner, float* kp_pool, int* kp_count, int max_kp, double feat_density,
                       double feat_dist_factor, double quality, int max_corners, FmTrackJob* jobs, float* scratch,
@@ -382,8 +384,9 @@ int fm_flow_keypoints(const unsigned char* prev_gray, int w, int h, const double
 /* The same for every cv2.goodFeaturesToTrack setting: block_size >= 1 (unnormalised box window anchored at
  * block_size / 2), gradient_size (Sobel aperture) 1 / 3 / 5 / 7, the minimum-eigenvalue response or, with use_harris,
  * a*c - b^2 - harris_k*(a+c)^2; max_corners <= 0 keeps every corner.  max_kp must hold min(max_corners, 4096) corners
- * (4096 when max_corners <= 0).  The default setting runs fm_flow_keypoints; the others use four scratch floats per
- * crop pixel. */
+ * (4096 when max_corners <= 0); a box that keeps more sets status 4.  The default setting runs fm_flow_keypoints; the
+ * others use four scratch floats per crop pixel, plus 4 per candidate, 2 per accepted corner and one per minDistance
+ * cell for a box with more than 4096 candidates. */
 int fm_flow_keypoints_cfg(const unsigned char* prev_gray, int w, int h, const double* tlbr_pool, const int* slots,
                           int n_trk, int* owner, float* kp_pool, int* kp_count, int max_kp, double feat_density,
                           double feat_dist_factor, double quality, int max_corners, int block_size, int gradient_size,
