@@ -79,10 +79,13 @@ class FmYoloHead(C.Structure):
     _fields_ = [("anchors", c_f * 12), ("scale_x_y", c_f)]
 
 
+class FmFrame(C.Structure):
+    _fields_ = [("y", c_p), ("uv", c_p), ("w", c_i), ("h", c_i), ("pitch", c_i), ("uv_pitch", c_i), ("format", c_i)]
+
+
 class FmFrameGeom(C.Structure):
-    _fields_ = [("frame", c_p), ("w", c_i), ("h", c_i), ("roi_x", c_i), ("roi_y", c_i), ("roi_w", c_i),
-                ("roi_h", c_i), ("size_w", c_f), ("size_h", c_f), ("off_x", c_f), ("off_y", c_f),
-                ("uv", c_p), ("pitch", c_i), ("uv_pitch", c_i), ("format", c_i)]
+    _fields_ = [("frame", FmFrame), ("roi_x", c_i), ("roi_y", c_i), ("roi_w", c_i), ("roi_h", c_i),
+                ("size_w", c_f), ("size_h", c_f), ("off_x", c_f), ("off_y", c_f)]
 
 
 FM_PIX_BGR, FM_PIX_NV12 = 0, 1
@@ -110,10 +113,8 @@ SIGNATURES = {
     "fm_greedy_match": (c_i, [c_p, c_i, c_i, c_d, c_p, c_p, c_p]),
     "fm_assoc_cascade": (c_i, [C.POINTER(FmCascadeDesc), c_p]),
     "fm_assoc_cascade_out_ints": (c_ll, [c_i]),
-    "fm_letterbox_preproc": (c_i, [c_p, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_p, c_p]),
-    "fm_roi_resize_norm": (c_i, [c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p]),
-    "fm_letterbox_preproc_nv12": (c_i, [c_p, c_p, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_p, c_p]),
-    "fm_roi_resize_norm_nv12": (c_i, [c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p]),
+    "fm_letterbox_preproc": (c_i, [C.POINTER(FmFrame), c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_p, c_p]),
+    "fm_roi_resize_norm": (c_i, [C.POINTER(FmFrame), c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p]),
     "fm_letterbox_preproc_geom": (c_i, [c_p, c_i, c_i, c_i, c_p, c_p]),
     "fm_roi_resize_norm_geom": (c_i, [c_p, c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p]),
     "fm_yolo_decode_filter_geom": (c_i, [c_p, c_i, c_ll, c_i, c_i, c_i, c_i, c_i, C.POINTER(FmYoloHead), c_i, c_i,
@@ -122,10 +123,8 @@ SIGNATURES = {
                                         c_p]),
     "fm_yolo_decode_filter": (c_i, [c_p, c_i, c_i, c_i, c_i, c_i, C.POINTER(FmYoloHead), c_i, c_i, c_i, c_i, c_i, c_p,
                                      c_d, c_f, c_f, c_f, c_f, c_p, c_p, c_p, c_i, c_p]),
-    "fm_gray_half": (c_i, [c_p, c_i, c_i, c_p, c_p, c_p]),
-    "fm_gray_resize": (c_i, [c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_p]),
-    "fm_gray_half_nv12": (c_i, [c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p, c_p]),
-    "fm_gray_resize_nv12": (c_i, [c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p, c_i, c_i, c_p]),
+    "fm_gray_half": (c_i, [C.POINTER(FmFrame), c_p, c_p, c_p]),
+    "fm_gray_resize": (c_i, [C.POINTER(FmFrame), c_p, c_p, c_i, c_i, c_p]),
     "fm_pyr_level": (c_i, [c_p, c_i, c_i, c_p, c_p]),
     "fm_scharr": (c_i, [c_p, c_i, c_i, c_p, c_p]),
     "fm_bg_small": (c_i, [c_p, c_p, c_i, c_i, c_p, c_p, c_i, c_i, c_p]),
@@ -142,10 +141,7 @@ SIGNATURES = {
                                               c_p, c_p, c_p, c_p, c_i, c_i, c_i, c_i, c_d, c_d, c_i, c_i, c_i, c_p]),
     "fm_flow_plan_create": (c_p, [C.POINTER(FmFlowPlan)]),
     "fm_flow_plan_destroy": (None, [c_p]),
-    "fm_flow_preprocess": (c_i, [c_p, c_p, c_i, c_p]),
-    "fm_flow_predict": (c_i, [c_p, c_p, c_i, c_i, c_p, c_p, c_p, c_p]),
-    "fm_flow_preprocess_nv12": (c_i, [c_p, c_p, c_p, c_i, c_i, c_i, c_p]),
-    "fm_flow_predict_nv12": (c_i, [c_p, c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p, c_p, c_p]),
+    "fm_flow_predict": (c_i, [c_p, C.POINTER(FmFrame), c_i, c_i, c_p, c_p, c_p, c_p]),
     "fm_conv2d_simt": (c_i, [C.POINTER(FmConvDesc), c_p, c_p, c_p, c_p, c_p, c_p]),
     "fm_maxpool": (c_i, [c_p, c_p, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_p]),
     "fm_maxpool_pad": (c_i, [c_p, c_p, c_i, c_i, c_i, c_i, c_i, c_i, c_i, c_p]),

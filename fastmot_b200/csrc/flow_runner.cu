@@ -118,37 +118,21 @@ extern "C" void fm_flow_plan_destroy(void* h) {
     } while (0)
 
 namespace {
-// the frame of one call: a BGR frame (uv == nullptr) or the two planes of an NV12 frame
-struct FrameIn {
-    const unsigned char* y;
-    const unsigned char* uv;
-    int y_pitch, uv_pitch;
-};
-
 // gray + optical-flow image + LK pyramid with Scharr derivatives for buffer k (flow.py:129-131 / :153-154).  An
 // optical-flow image of exactly half the frame in both directions is the 2x2 mean (what cv2.resize computes there);
 // any other size is the general INTER_LINEAR resize.
-int preprocess(FlowRunner* r, const FrameIn& f, int k, void* stream) {
+int preprocess(FlowRunner* r, const FmFrame* f, int k, void* stream) {
     const FmFlowPlan& p = r->p;
     const FmPyramid& py = p.pyr[k];
     unsigned char* small = (unsigned char*)py.img[0];
-    if (2 * py.w[0] == p.frame_w && 2 * py.h[0] == p.frame_h) {
-        if (f.uv)
-            FM_TRY(fm_gray_half_nv12(f.y, f.uv, f.y_pitch, f.uv_pitch, p.frame_w, p.frame_h, p.gray[k], small,
-                                     stream));
-        else
-            FM_TRY(fm_gray_half(f.y, p.frame_w, p.frame_h, p.gray[k], small, stream));
-    } else {
-        if (f.uv)
-            FM_TRY(fm_gray_resize_nv12(f.y, f.uv, f.y_pitch, f.uv_pitch, p.frame_w, p.frame_h, p.gray[k], small,
-                                       py.w[0], py.h[0], stream));
-        else
-            FM_TRY(fm_gray_resize(f.y, p.frame_w, p.frame_h, p.gray[k], small, py.w[0], py.h[0], stream));
-    }
+    if (2 * py.w[0] == p.frame_w && 2 * py.h[0] == p.frame_h)
+        FM_TRY(fm_gray_half(f, p.gray[k], small, stream));
+    else
+        FM_TRY(fm_gray_resize(f, p.gray[k], small, py.w[0], py.h[0], stream));
     if (pyr_graph_enabled()) {
         if (r->pyr_state[k] == 0) build_pyr_graph(r, k);
         if (r->pyr_state[k] == 1) {
-            FM_CUDA_TRY(cudaGraphLaunch(r->pyr_graph[k], (cudaStream_t)stream), "fm_flow_preprocess: pyramid graph");
+            FM_CUDA_TRY(cudaGraphLaunch(r->pyr_graph[k], (cudaStream_t)stream), "fm_flow_predict: pyramid graph");
             fm_count_launches(r->pyr_nodes);
             return FM_OK;
         }
@@ -161,7 +145,7 @@ int preprocess(FlowRunner* r, const FrameIn& f, int k, void* stream) {
     return FM_OK;
 }
 
-int predict(FlowRunner* r, const FrameIn& f, int prev, int n_trk, double* H_out, int* h_ok, void* s_main,
+int predict(FlowRunner* r, const FmFrame* f, int prev, int n_trk, double* H_out, int* h_ok, void* s_main,
             void* s_side) {
     const FmFlowPlan& p = r->p;
     const int cur = 1 - prev;
@@ -197,32 +181,12 @@ int predict(FlowRunner* r, const FrameIn& f, int prev, int n_trk, double* H_out,
 }
 }  // namespace
 
-extern "C" int fm_flow_preprocess(void* h, const unsigned char* frame, int k, void* stream) {
-    FlowRunner* r = (FlowRunner*)h;
-    FM_REQUIRE(r && frame && (k == 0 || k == 1), "fm_flow_preprocess: bad handle / frame / buffer index");
-    return preprocess(r, FrameIn{frame, nullptr, 0, 0}, k, stream);
-}
-
-extern "C" int fm_flow_preprocess_nv12(void* h, const unsigned char* y, const unsigned char* uv, int y_pitch,
-                                       int uv_pitch, int k, void* stream) {
-    FlowRunner* r = (FlowRunner*)h;
-    FM_REQUIRE(r && y && uv && (k == 0 || k == 1), "fm_flow_preprocess_nv12: bad handle / planes / buffer index");
-    return preprocess(r, FrameIn{y, uv, y_pitch, uv_pitch}, k, stream);
-}
-
-extern "C" int fm_flow_predict(void* h, const unsigned char* frame, int prev, int n_trk, double* H_out, int* h_ok,
+extern "C" int fm_flow_predict(void* h, const FmFrame* frame, int prev, int n_trk, double* H_out, int* h_ok,
                                void* s_main, void* s_side) {
     FlowRunner* r = (FlowRunner*)h;
     FM_REQUIRE(r && frame && (prev == 0 || prev == 1) && n_trk >= 0 && H_out && h_ok,
                "fm_flow_predict: bad handle / frame / buffer index / track count");
-    return predict(r, FrameIn{frame, nullptr, 0, 0}, prev, n_trk, H_out, h_ok, s_main, s_side);
-}
-
-extern "C" int fm_flow_predict_nv12(void* h, const unsigned char* y, const unsigned char* uv, int y_pitch,
-                                    int uv_pitch, int prev, int n_trk, double* H_out, int* h_ok, void* s_main,
-                                    void* s_side) {
-    FlowRunner* r = (FlowRunner*)h;
-    FM_REQUIRE(r && y && uv && (prev == 0 || prev == 1) && n_trk >= 0 && H_out && h_ok,
-               "fm_flow_predict_nv12: bad handle / planes / buffer index / track count");
-    return predict(r, FrameIn{y, uv, y_pitch, uv_pitch}, prev, n_trk, H_out, h_ok, s_main, s_side);
+    FM_REQUIRE(frame->w == r->p.frame_w && frame->h == r->p.frame_h,
+               "fm_flow_predict: the frame is not the plan's frame_w x frame_h");
+    return predict(r, frame, prev, n_trk, H_out, h_ok, s_main, s_side);
 }

@@ -1,6 +1,6 @@
 // KLT image pyramid kernels (byte work, HBM/L2-bound): BGR->gray + 0.5x box mean in one pass, BGR->gray + an
-// INTER_LINEAR resize to any optical-flow size (both also reading NV12 frames in place, pixel_src.cuh), 5-tap Gaussian pyrDown, int16 Scharr derivatives, 0.1x background
-// image + mask.
+// INTER_LINEAR resize to any optical-flow size (both also reading NV12 frames in place, pixel_src.cuh), 5-tap Gaussian
+// pyrDown, int16 Scharr derivatives, 0.1x background image + mask.
 //
 // Reference: fastmot/flow.py:121-133, 153-154, 187-189 (cv2.cvtColor / cv2.resize) and the pyramid that
 // cv2.calcOpticalFlowPyrLK builds internally (flow.py:203-207; OpenCV lkpyramid.cpp: buildOpticalFlowPyramid,
@@ -158,54 +158,33 @@ __global__ void bg_small_kernel(const unsigned char* __restrict__ gray, const in
 
 }  // namespace
 
-namespace {
-template <class Src>
-int gray_half_launch(const char* name, Src src, int w, int h, unsigned char* gray, unsigned char* small, void* stream) {
+extern "C" int fm_gray_half(const FmFrame* frame, unsigned char* gray, unsigned char* small, void* stream) {
+    FM_REQUIRE(frame && fm_frame_ok(*frame), "fm_gray_half: " FM_FRAME_RULES);
+    const int w = frame->w, h = frame->h;
     const int sw = (w + 1) / 2, sh = (h + 1) / 2;
     FM_REQUIRE(w % 2 == 0 && h % 2 == 0, "fm_gray_half: frame size must be even (0.5x resize = 2x2 mean)");
-    dim3 grid(fm_cdiv(sw, 256), sh);
-    gray_half_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(src, w, h, gray, small, sw, sh);
-    FM_CHECK_LAUNCH(name);
+    const dim3 grid(fm_cdiv(sw, 256), sh);
+    fm_visit_src(*frame, [&](auto src) {
+        gray_half_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(src, w, h, gray, small, sw, sh);
+    });
+    FM_CHECK_LAUNCH("fm_gray_half");
     return FM_OK;
 }
 
-template <class Src>
-int gray_resize_launch(const char* name, Src src, int w, int h, unsigned char* gray, unsigned char* small, int sw,
-                       int sh, void* stream) {
-    FM_REQUIRE(w > 0 && h > 0 && sw > 0 && sh > 0 && sw <= w && sh <= h,
+extern "C" int fm_gray_resize(const FmFrame* frame, unsigned char* gray, unsigned char* small, int sw, int sh,
+                              void* stream) {
+    FM_REQUIRE(frame && fm_frame_ok(*frame), "fm_gray_resize: " FM_FRAME_RULES);
+    const int w = frame->w, h = frame->h;
+    FM_REQUIRE(sw > 0 && sh > 0 && sw <= w && sh <= h,
                "fm_gray_resize: the optical-flow image must be non-empty and no larger than the frame");
-    gray_kernel<<<dim3(fm_cdiv(w, 256), h), 256, 0, (cudaStream_t)stream>>>(src, w, h, gray);
+    fm_visit_src(*frame, [&](auto src) {
+        gray_kernel<<<dim3(fm_cdiv(w, 256), h), 256, 0, (cudaStream_t)stream>>>(src, w, h, gray);
+    });
     resize_linear_kernel<<<dim3(fm_cdiv(sw, 256), sh), 256, 0, (cudaStream_t)stream>>>(
         gray, w, h, small, sw, sh, 1.0 / ((double)sw / w), 1.0 / ((double)sh / h));
     fm_count_launches(1);
-    FM_CHECK_LAUNCH(name);
+    FM_CHECK_LAUNCH("fm_gray_resize");
     return FM_OK;
-}
-}  // namespace
-
-extern "C" int fm_gray_half(const unsigned char* frame, int w, int h, unsigned char* gray, unsigned char* small,
-                            void* stream) {
-    return gray_half_launch("fm_gray_half", BgrSrc{frame, w}, w, h, gray, small, stream);
-}
-
-extern "C" int fm_gray_half_nv12(const unsigned char* y, const unsigned char* uv, int y_pitch, int uv_pitch, int w,
-                                 int h, unsigned char* gray, unsigned char* small, void* stream) {
-    FM_REQUIRE(fm_nv12_ok(y, uv, y_pitch, uv_pitch, w, h),
-               "fm_gray_half_nv12: NV12 needs even w, h > 0, both planes and pitches >= w");
-    return gray_half_launch("fm_gray_half_nv12", Nv12Src{y, uv, y_pitch, uv_pitch}, w, h, gray, small, stream);
-}
-
-extern "C" int fm_gray_resize(const unsigned char* frame, int w, int h, unsigned char* gray, unsigned char* small,
-                              int sw, int sh, void* stream) {
-    return gray_resize_launch("fm_gray_resize", BgrSrc{frame, w}, w, h, gray, small, sw, sh, stream);
-}
-
-extern "C" int fm_gray_resize_nv12(const unsigned char* y, const unsigned char* uv, int y_pitch, int uv_pitch, int w,
-                                   int h, unsigned char* gray, unsigned char* small, int sw, int sh, void* stream) {
-    FM_REQUIRE(fm_nv12_ok(y, uv, y_pitch, uv_pitch, w, h),
-               "fm_gray_resize_nv12: NV12 needs even w, h > 0, both planes and pitches >= w");
-    return gray_resize_launch("fm_gray_resize_nv12", Nv12Src{y, uv, y_pitch, uv_pitch}, w, h, gray, small, sw, sh,
-                              stream);
 }
 
 extern "C" int fm_pyr_level(const unsigned char* src, int sw, int sh, unsigned char* dst, void* stream) {

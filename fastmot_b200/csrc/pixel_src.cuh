@@ -6,6 +6,7 @@
 //             20 fractional bits, chroma of the pixel's 2x2 block (nearest neighbour).  Pinned against cv2 on all
 //             2^24 (Y, U, V) triples by tests/test_nv12_cpu.py through the restatement in oracle/nv12.py.
 #pragma once
+#include "../../include/fastmot_b200.h"
 
 __device__ __forceinline__ int fm_clamp_u8(int v) { return v < 0 ? 0 : v > 255 ? 255 : v; }
 
@@ -36,7 +37,19 @@ struct Nv12Src {
     }
 };
 
-// what every NV12 entry point requires of its frame
-static inline bool fm_nv12_ok(const void* y, const void* uv, int y_pitch, int uv_pitch, int w, int h) {
-    return y && uv && w > 0 && h > 0 && w % 2 == 0 && h % 2 == 0 && y_pitch >= w && uv_pitch >= w;
+// The pixel source of an FmFrame: returns f(BgrSrc{...}) or f(Nv12Src{...}) (an NV12 pitch of 0 means w).
+template <class F>
+__host__ __device__ __forceinline__ auto fm_visit_src(const FmFrame& fr, F&& f) {
+    if (fr.format == FM_PIX_NV12)
+        return f(Nv12Src{fr.y, fr.uv, fr.pitch ? fr.pitch : fr.w, fr.uv_pitch ? fr.uv_pitch : fr.w});
+    return f(BgrSrc{fr.y, fr.w});
 }
+
+// what every one-frame entry point requires of its frame (include/fastmot_b200.h: FmFrame)
+static inline bool fm_frame_ok(const FmFrame& f) {
+    if (!f.y || f.w <= 0 || f.h <= 0) return false;
+    if (f.format == FM_PIX_BGR) return true;
+    return f.format == FM_PIX_NV12 && f.uv && f.w % 2 == 0 && f.h % 2 == 0 && (f.pitch == 0 || f.pitch >= f.w) &&
+           (f.uv_pitch == 0 || f.uv_pitch >= f.w);
+}
+#define FM_FRAME_RULES "a BGR frame needs y and w, h > 0; an NV12 frame both planes, even w, h > 0 and pitches >= w"

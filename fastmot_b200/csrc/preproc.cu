@@ -4,10 +4,10 @@
 //   fm_roi_resize_norm   : per-detection crop + OpenCV-style fixed-point bilinear resize to 128x256 + ImageNet
 //                          normalisation, all crops in one launch (fastmot/feature_extractor.py:48-60, 84-98;
 //                          fastmot/utils/rect.py:92-97)
-// The *_geom entries read each frame's pointer, size, pixel format (and, for the letterbox, ROI) from a device
+// Both read a BGR or an NV12 frame (FmFrame) in place; an NV12 bilinear tap is converted to BGR before it is
+// interpolated (pixel_src.cuh).  The *_geom entries read each frame (and, for the letterbox, its ROI) from a device
 // FmFrameGeom table (one grid slice per frame, or one frame index per crop), so one launch covers several frames of
-// any sizes and formats; every pixel is computed by the same body as in the one-frame entries.  The *_nv12 entries
-// read an NV12 frame in place (pixel_src.cuh): each bilinear tap is converted to BGR before it is interpolated.
+// any sizes and formats; every pixel is computed by the same body as in the one-frame entries.
 // Outputs are either fp32 planar CHW (the reference's TensorRT input layout; used for parity tests) or fp16
 // NHWC with C padded to 8 (one 16-byte chunk per pixel; what the conv engine consumes).
 #include "common.cuh"
@@ -90,12 +90,10 @@ __global__ void __launch_bounds__(256) letterbox_geom_kernel(const FmFrameGeom* 
     if (x >= dst_w) return;
     const FmFrameGeom& g = geom[blockIdx.z];
     out = (__half*)out + (size_t)blockIdx.z * dst_h * dst_w * 8;
-    if (g.format == FM_PIX_NV12)
-        letterbox_px<1>(Nv12Src{g.frame, g.uv, g.pitch ? g.pitch : g.w, g.uv_pitch ? g.uv_pitch : g.w}, g.w, g.h,
-                        dst_w, dst_h, g.roi_x, g.roi_y, g.roi_w, g.roi_h, out, x, blockIdx.y);
-    else
-        letterbox_px<1>(BgrSrc{g.frame, g.w}, g.w, g.h, dst_w, dst_h, g.roi_x, g.roi_y, g.roi_w, g.roi_h, out, x,
+    fm_visit_src(g.frame, [&](const auto& src) {
+        letterbox_px<1>(src, g.frame.w, g.frame.h, dst_w, dst_h, g.roi_x, g.roi_y, g.roi_w, g.roi_h, out, x,
                         blockIdx.y);
+    });
 }
 
 // OpenCV INTER_LINEAR for 8-bit: 11-bit fixed-point coefficients, horizontal pass in int, vertical pass
@@ -171,83 +169,54 @@ __global__ void __launch_bounds__(128) roi_resize_norm_geom_kernel(const FmFrame
     if (crop >= n) return;
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     if (x >= out_w) return;
-    const FmFrameGeom& g = geom[frame_idx[crop]];
-    if (g.format == FM_PIX_NV12)
-        roi_px<LAYOUT>(Nv12Src{g.frame, g.uv, g.pitch ? g.pitch : g.w, g.uv_pitch ? g.uv_pitch : g.w}, g.w, g.h,
-                       tlbrs, crop, out_w, out_h, out, x, blockIdx.y);
-    else
-        roi_px<LAYOUT>(BgrSrc{g.frame, g.w}, g.w, g.h, tlbrs, crop, out_w, out_h, out, x, blockIdx.y);
+    const FmFrame& f = geom[frame_idx[crop]].frame;
+    fm_visit_src(f, [&](const auto& src) {
+        roi_px<LAYOUT>(src, f.w, f.h, tlbrs, crop, out_w, out_h, out, x, blockIdx.y);
+    });
 }
 
 }  // namespace
 
-namespace {
-template <class Src>
-int letterbox_launch(const char* name, Src src, int src_w, int src_h, int dst_w, int dst_h, int roi_x, int roi_y,
-                     int roi_w, int roi_h, int layout, void* out, void* stream) {
+extern "C" int fm_letterbox_preproc(const FmFrame* frame, int dst_w, int dst_h, int roi_x, int roi_y, int roi_w,
+                                    int roi_h, int layout, void* out, void* stream) {
+    FM_REQUIRE(frame && fm_frame_ok(*frame), "fm_letterbox_preproc: " FM_FRAME_RULES);
     FM_REQUIRE(layout == 0 || layout == 1, "fm_letterbox_preproc: layout must be 0 (f32 CHW) or 1 (f16 NHWC8)");
     FM_REQUIRE(roi_w > 0 && roi_h > 0, "fm_letterbox_preproc: empty ROI");
-    dim3 grid(fm_cdiv(dst_w, 256), dst_h);
-    if (layout == 0)
-        letterbox_kernel<0><<<grid, 256, 0, (cudaStream_t)stream>>>(src, src_w, src_h, dst_w, dst_h, roi_x, roi_y,
-                                                                    roi_w, roi_h, out);
-    else
-        letterbox_kernel<1><<<grid, 256, 0, (cudaStream_t)stream>>>(src, src_w, src_h, dst_w, dst_h, roi_x, roi_y,
-                                                                    roi_w, roi_h, out);
-    FM_CHECK_LAUNCH(name);
+    const dim3 grid(fm_cdiv(dst_w, 256), dst_h);
+    const int w = frame->w, h = frame->h;
+    fm_visit_src(*frame, [&](auto src) {
+        if (layout == 0)
+            letterbox_kernel<0><<<grid, 256, 0, (cudaStream_t)stream>>>(src, w, h, dst_w, dst_h, roi_x, roi_y, roi_w,
+                                                                        roi_h, out);
+        else
+            letterbox_kernel<1><<<grid, 256, 0, (cudaStream_t)stream>>>(src, w, h, dst_w, dst_h, roi_x, roi_y, roi_w,
+                                                                        roi_h, out);
+    });
+    FM_CHECK_LAUNCH("fm_letterbox_preproc");
     return FM_OK;
 }
 
-template <class Src>
-int roi_launch(const char* name, Src src, int src_w, int src_h, const double* tlbrs, const int* n_dev, int n_max,
-               int out_w, int out_h, int layout, void* out, void* stream) {
+extern "C" int fm_roi_resize_norm(const FmFrame* frame, const double* tlbrs, const int* n_dev, int n_max, int out_w,
+                                  int out_h, int layout, void* out, void* stream) {
+    FM_REQUIRE(frame && fm_frame_ok(*frame), "fm_roi_resize_norm: " FM_FRAME_RULES);
     FM_REQUIRE(layout >= 0 && layout <= 2, "fm_roi_resize_norm: layout must be 0 (f32 CHW), 1 (f16 NHWC8) or 2 (f16 NHWC4, padded)");
     if (n_max <= 0) return FM_OK;
     FM_REQUIRE(n_max <= 65535, "fm_roi_resize_norm: more than 65535 crops");
-    dim3 grid(fm_cdiv(out_w, 128), out_h, n_max);
-    if (layout == 0)
-        roi_resize_norm_kernel<0><<<grid, 128, 0, (cudaStream_t)stream>>>(src, src_w, src_h, tlbrs, n_dev, n_max,
-                                                                          out_w, out_h, out);
-    else if (layout == 1)
-        roi_resize_norm_kernel<1><<<grid, 128, 0, (cudaStream_t)stream>>>(src, src_w, src_h, tlbrs, n_dev, n_max,
-                                                                          out_w, out_h, out);
-    else
-        roi_resize_norm_kernel<2><<<grid, 128, 0, (cudaStream_t)stream>>>(src, src_w, src_h, tlbrs, n_dev, n_max,
-                                                                          out_w, out_h, out);
-    FM_CHECK_LAUNCH(name);
+    const dim3 grid(fm_cdiv(out_w, 128), out_h, n_max);
+    const int w = frame->w, h = frame->h;
+    fm_visit_src(*frame, [&](auto src) {
+        if (layout == 0)
+            roi_resize_norm_kernel<0><<<grid, 128, 0, (cudaStream_t)stream>>>(src, w, h, tlbrs, n_dev, n_max, out_w,
+                                                                              out_h, out);
+        else if (layout == 1)
+            roi_resize_norm_kernel<1><<<grid, 128, 0, (cudaStream_t)stream>>>(src, w, h, tlbrs, n_dev, n_max, out_w,
+                                                                              out_h, out);
+        else
+            roi_resize_norm_kernel<2><<<grid, 128, 0, (cudaStream_t)stream>>>(src, w, h, tlbrs, n_dev, n_max, out_w,
+                                                                              out_h, out);
+    });
+    FM_CHECK_LAUNCH("fm_roi_resize_norm");
     return FM_OK;
-}
-}  // namespace
-
-extern "C" int fm_letterbox_preproc(const unsigned char* frame, int src_w, int src_h, int dst_w, int dst_h,
-                                    int roi_x, int roi_y, int roi_w, int roi_h, int layout, void* out, void* stream) {
-    return letterbox_launch("fm_letterbox_preproc", BgrSrc{frame, src_w}, src_w, src_h, dst_w, dst_h, roi_x, roi_y,
-                            roi_w, roi_h, layout, out, stream);
-}
-
-extern "C" int fm_letterbox_preproc_nv12(const unsigned char* y, const unsigned char* uv, int y_pitch, int uv_pitch,
-                                         int src_w, int src_h, int dst_w, int dst_h, int roi_x, int roi_y, int roi_w,
-                                         int roi_h, int layout, void* out, void* stream) {
-    FM_REQUIRE(fm_nv12_ok(y, uv, y_pitch, uv_pitch, src_w, src_h),
-               "fm_letterbox_preproc_nv12: NV12 needs even w, h > 0, both planes and pitches >= w");
-    return letterbox_launch("fm_letterbox_preproc_nv12", Nv12Src{y, uv, y_pitch, uv_pitch}, src_w, src_h, dst_w,
-                            dst_h, roi_x, roi_y, roi_w, roi_h, layout, out, stream);
-}
-
-extern "C" int fm_roi_resize_norm(const unsigned char* frame, int src_w, int src_h, const double* tlbrs,
-                                  const int* n_dev, int n_max, int out_w, int out_h, int layout, void* out,
-                                  void* stream) {
-    return roi_launch("fm_roi_resize_norm", BgrSrc{frame, src_w}, src_w, src_h, tlbrs, n_dev, n_max, out_w, out_h,
-                      layout, out, stream);
-}
-
-extern "C" int fm_roi_resize_norm_nv12(const unsigned char* y, const unsigned char* uv, int y_pitch, int uv_pitch,
-                                       int src_w, int src_h, const double* tlbrs, const int* n_dev, int n_max,
-                                       int out_w, int out_h, int layout, void* out, void* stream) {
-    FM_REQUIRE(fm_nv12_ok(y, uv, y_pitch, uv_pitch, src_w, src_h),
-               "fm_roi_resize_norm_nv12: NV12 needs even w, h > 0, both planes and pitches >= w");
-    return roi_launch("fm_roi_resize_norm_nv12", Nv12Src{y, uv, y_pitch, uv_pitch}, src_w, src_h, tlbrs, n_dev,
-                      n_max, out_w, out_h, layout, out, stream);
 }
 
 extern "C" int fm_letterbox_preproc_geom(const FmFrameGeom* geom, int batch, int dst_w, int dst_h, void* out,

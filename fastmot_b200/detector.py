@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _lib, models
-from .devmem import ptr, stream_ptr, FrameUploader, Frame, nv12_frame
+from .devmem import ptr, stream_ptr, device_frame, FrameUploader, UploadSlot
 from .models.yolo import check_heads
 
 DET_DTYPE = np.dtype(
@@ -133,8 +133,8 @@ class YOLODetector(Detector):
         self._h_meta = torch.zeros(max(4, 3 * B), dtype=torch.int32).pin_memory()
         lead = () if B == 1 else (B,)
         self.inp = torch.zeros(lead + (in_h, in_w, 8), dtype=torch.float16, device=dev)   # NHWC8
-        self._uploader = FrameUploader(size)
-        self._uploaders = [self._uploader] + [None] * (B - 1)    # built on the first host frame of their slot
+        # host frames of image b go through slot b
+        self._uploads = [UploadSlot(FrameUploader(size))] + [UploadSlot() for _ in range(B - 1)]
         # per-frame geometry of detect_batch_async (one FmFrameGeom row per image)
         self._geom_bytes = C.sizeof(_lib.FmFrameGeom)
         self._geom_h = torch.zeros(B * self._geom_bytes, dtype=torch.uint8).pin_memory()
@@ -158,28 +158,16 @@ class YOLODetector(Detector):
     def preprocess(self, frame_dev):
         """fastmot/detector.py:289-300 on the device (frame_dev: HxWx3 u8 cuda tensor, or a device Frame of this
         detector's size: an NV12 frame is read in place)."""
+        f = device_frame(frame_dev, size=self.size)
         rx, ry, rw, rh = self.roi
-        if isinstance(frame_dev, Frame) and frame_dev.format == "NV12":
-            if frame_dev.size != tuple(self.size):
-                raise ValueError(f"frame of size {frame_dev.size}, the detector's is {tuple(self.size)}")
-            rc = self._lib.fm_letterbox_preproc_nv12(*frame_dev.nv12_args(), self.size[0], self.size[1],
-                                                     self.input_wh[0], self.input_wh[1], rx, ry, rw, rh, 1,
-                                                     ptr(self.inp), stream_ptr())
-            _lib.check(rc, "fm_letterbox_preproc_nv12")
-            return
-        if isinstance(frame_dev, Frame):
-            frame_dev = frame_dev.y
-        rc = self._lib.fm_letterbox_preproc(ptr(frame_dev), self.size[0], self.size[1], self.input_wh[0],
-                                            self.input_wh[1], rx, ry, rw, rh, 1, ptr(self.inp), stream_ptr())
+        rc = self._lib.fm_letterbox_preproc(C.byref(f.fm()), self.input_wh[0], self.input_wh[1], rx, ry, rw, rh, 1,
+                                            ptr(self.inp), stream_ptr())
         _lib.check(rc, "fm_letterbox_preproc")
 
     def detect_async(self, frame):
         """Upload (if `frame` is a host array or a host NV12 Frame), pre-process, run the conv stack and the whole
         post-processing asynchronously; `postprocess` waits for the D result rows."""
-        if isinstance(frame, Frame):
-            self.frame_dev = self._device(0, frame)
-        else:
-            self.frame_dev = frame if torch.is_tensor(frame) else self._uploader.upload(frame)
+        self.frame_dev = device_frame(frame, self._uploads[0])
         self.preprocess(self.frame_dev)
         heads = self.backend.forward(self.inp)
         self.postprocess_heads_async(heads)
@@ -247,7 +235,7 @@ class YOLODetector(Detector):
         k = len(frames)
         if not 1 <= k <= self.batch:
             raise ValueError(f"expected 1 to {self.batch} frames, got {k}")
-        self.frames_dev = [self._device(b, f) for b, f in enumerate(frames)]
+        self.frames_dev = [device_frame(f, up) for f, up in zip(frames, self._uploads)]
         geom = self.preprocess_frames(self.frames_dev)
         # a batch-1 input has no image dimension, in this detector and in its batch-1 engine
         inp = self.inp if self.batch == 1 else self.inp[:k] if k > 1 else self.inp[0]
@@ -268,22 +256,6 @@ class YOLODetector(Detector):
         for k in range(1, self.batch + 1):
             self.engine(k)
 
-    def _device(self, b, frame):
-        """Frame b of a call on the device: cuda tensors and device Frames pass through, host frames (HxWx3 ndarrays,
-        host NV12 Frames) go through upload slot b."""
-        if torch.is_tensor(frame) or (isinstance(frame, Frame) and frame.on_device):
-            return frame
-        return self._upload(b, frame)
-
-    def _upload(self, b, frame):
-        fmt = frame.format if isinstance(frame, Frame) else "BGR"
-        (w, h), host = (frame.size, frame.y) if isinstance(frame, Frame) else ((frame.shape[1], frame.shape[0]), frame)
-        up = self._uploaders[b]
-        if up is None or up.pixel_format != fmt or up.shape != FrameUploader.frame_shape((w, h), fmt):
-            self._uploaders[b] = up = FrameUploader((w, h), pixel_format=fmt)
-        t = up.upload(host)
-        return nv12_frame(t) if fmt == "NV12" else t
-
     def geometry(self, wh):
         """(roi, upscaled_sz, bbox_offset) of frames of size wh = (width, height) in this detector's input."""
         wh = tuple(int(v) for v in wh)
@@ -299,8 +271,7 @@ class YOLODetector(Detector):
         for b, (r, (w, h)) in enumerate(zip(rows, sizes)):
             (rx, ry, rw, rh), up, off = self.geometry((w, h))
             if frames is not None:
-                frames[b].fill_geom(r)
-            r.w, r.h = w, h
+                r.frame = frames[b].fm()
             r.roi_x, r.roi_y, r.roi_w, r.roi_h = rx, ry, rw, rh
             r.size_w, r.size_h, r.off_x, r.off_y = float(up[0]), float(up[1]), float(off[0]), float(off[1])
         if self._geom_ev is not None:
@@ -318,7 +289,7 @@ class YOLODetector(Detector):
         k = len(frames_dev)
         if not 1 <= k <= self.batch:
             raise ValueError(f"expected 1 to {self.batch} frames, got {k}")
-        frames = [f if isinstance(f, Frame) and f.on_device else Frame.bgr(f) for f in frames_dev]
+        frames = [device_frame(f) for f in frames_dev]
         geom = self._upload_geom([f.size for f in frames], frames)
         rc = self._lib.fm_letterbox_preproc_geom(ptr(geom), k, self.input_wh[0], self.input_wh[1], ptr(self.inp),
                                                  stream_ptr())

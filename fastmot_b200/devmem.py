@@ -8,6 +8,8 @@ import ctypes as C
 import numpy as np
 import torch
 
+from . import _lib
+
 
 def ptr(t):
     """Raw device (or pinned-host) address of a torch tensor, or None."""
@@ -119,15 +121,16 @@ class Frame:
 
     BGR: `y` is an HxWx3 uint8 cuda tensor (tight rows); `uv` is None.
     NV12 (hardware video decoders): `y` is the H x W luma plane and `uv` the H/2 x W plane of interleaved U, V at half
-    resolution, each with its own row pitch in bytes (`y_pitch`, `uv_pitch` >= W).  A host NV12 frame (`on_device`
-    False) holds its (3H/2, W) ndarray in `y`; FrameUploader turns it into a device frame.  Build NV12 frames with
+    resolution, each with its own row pitch in bytes (`y_pitch`, `uv_pitch` >= W).  Build NV12 frames with
     `nv12_frame`; the planes are views of the caller's memory, nothing is copied.
+    A host frame (`on_device` False) holds its ndarray in `y` (HxWx3 BGR or (3H/2, W) NV12); `device_frame` uploads it.
     """
-    __slots__ = ("format", "w", "h", "y", "uv", "y_pitch", "uv_pitch")
+    __slots__ = ("format", "w", "h", "y", "uv", "y_pitch", "uv_pitch", "_fm")
 
     def __init__(self, format, w, h, y, uv=None, y_pitch=0, uv_pitch=0):
         self.format, self.w, self.h = format, int(w), int(h)
         self.y, self.uv, self.y_pitch, self.uv_pitch = y, uv, int(y_pitch), int(uv_pitch)
+        self._fm = None
 
     @classmethod
     def bgr(cls, t):
@@ -145,18 +148,14 @@ class Frame:
     def on_device(self):
         return torch.is_tensor(self.y)
 
-    def nv12_args(self):
-        """(y, uv, y_pitch, uv_pitch) for the *_nv12 entry points."""
-        return ptr(self.y), ptr(self.uv), self.y_pitch, self.uv_pitch
-
-    def fill_geom(self, row):
-        """Writes the frame fields of one FmFrameGeom row (pointer, size, format)."""
-        from . import _lib
-        row.frame, row.w, row.h = self.y.data_ptr(), self.w, self.h
-        if self.format == "NV12":
-            row.uv, row.pitch, row.uv_pitch, row.format = self.uv.data_ptr(), self.y_pitch, self.uv_pitch, _lib.FM_PIX_NV12
-        else:
-            row.uv, row.pitch, row.uv_pitch, row.format = None, 0, 0, _lib.FM_PIX_BGR
+    def fm(self):
+        """The FmFrame of this device frame, which every C entry point that reads camera pixels takes (built on the
+        first call).  It holds raw plane addresses: keep this Frame referenced until the kernels that read them ran."""
+        if self._fm is None:
+            nv12 = self.format == "NV12"
+            self._fm = _lib.FmFrame(self.y.data_ptr(), self.uv.data_ptr() if nv12 else None, self.w, self.h,
+                                    self.y_pitch, self.uv_pitch, _lib.FM_PIX_NV12 if nv12 else _lib.FM_PIX_BGR)
+        return self._fm
 
 
 def _plane(t, rows, w, what):
@@ -237,7 +236,6 @@ class FrameUploader:
     directly; pageable ones are staged through an internal pinned ring."""
 
     def __init__(self, size, depth=2, device="cuda", pixel_format="BGR"):
-        from . import _lib
         self._lib = _lib.load()
         self.pixel_format = check_pixel_format(pixel_format)
         self.shape = self.frame_shape(size, self.pixel_format)
@@ -316,16 +314,61 @@ class FrameUploader:
         self._copy(frame, k, torch.cuda.current_stream())
         return self.dev[k]
 
+    def upload_frame(self, f):
+        """A host Frame of this uploader's format and size -> its device Frame."""
+        t = self.upload(f.y)
+        return nv12_frame(t) if self.pixel_format == "NV12" else Frame.bgr(t)
 
-def device_frame(frame, pixel_format, uploader):
-    """A caller's frame as the stages take it: BGR -- the cuda tensor itself, or the uploaded HxWx3 host array; NV12 --
-    the device Frame of any form nv12_frame accepts, host frames uploaded through `uploader` (an NV12 FrameUploader of
-    the frame's size)."""
-    if pixel_format == "BGR":
-        return frame if torch.is_tensor(frame) else uploader.upload(frame)
-    f = nv12_frame(frame)
+
+class UploadSlot:
+    """Uploads host Frames of any format and size: keeps the FrameUploader of the last one and builds a new one when the
+    format or size changes (a stage used on its own, whose caller may change the frame size between calls)."""
+
+    def __init__(self, uploader=None):
+        self.uploader = uploader
+
+    def upload_frame(self, f):
+        up = self.uploader
+        if up is None or up.pixel_format != f.format or up.shape != FrameUploader.frame_shape(f.size, f.format):
+            self.uploader = up = FrameUploader(f.size, pixel_format=f.format)
+        return up.upload_frame(f)
+
+
+def as_frame(frame, pixel_format="BGR", size=None):
+    """A caller's frame as a Frame, nothing copied.  A Frame passes through; otherwise `frame` is in pixel_format:
+    'BGR' -- an HxWx3 uint8 cuda tensor (contiguous) or host ndarray; 'NV12' -- any form nv12_frame accepts.  size:
+    the (width, height) the frame must have; another size raises ValueError."""
+    if isinstance(frame, Frame):
+        f = frame
+    elif pixel_format == "NV12":
+        f = nv12_frame(frame)
+    elif torch.is_tensor(frame):
+        f = Frame.bgr(frame)
+    else:
+        if not (isinstance(frame, np.ndarray) and frame.dtype == np.uint8 and frame.ndim == 3 and frame.shape[2] == 3):
+            raise ValueError(f"BGR host frame: expected an HxWx3 uint8 ndarray, got {type(frame).__name__} "
+                             f"{getattr(frame, 'dtype', '')} {getattr(frame, 'shape', '')}")
+        f = Frame("BGR", frame.shape[1], frame.shape[0], frame)
+    if size is not None and f.size != tuple(size):
+        raise ValueError(f"{f.format} frame of size {f.size}, expected {tuple(size)}")
+    return f
+
+
+def device_frame(frame, uploader=None, pixel_format="BGR", size=None):
+    """The device Frame of a caller's frame (any input as_frame takes, checked against `size` as there).  A host frame
+    is uploaded through `uploader`: a FrameUploader of its format and size, or an UploadSlot; without one a host frame
+    raises ValueError."""
+    f = as_frame(frame, pixel_format, size)
     if f.on_device:
         return f
-    if f.size != (uploader.shape[1], uploader.shape[0] * 2 // 3):
-        raise ValueError(f"NV12 frame of size {f.size}, expected {(uploader.shape[1], uploader.shape[0] * 2 // 3)}")
-    return nv12_frame(uploader.upload(f.y))
+    if uploader is None:
+        raise ValueError("expected a frame in device memory, got a host frame")
+    return uploader.upload_frame(f)
+
+
+def prefetch_frame(frame, uploader, pixel_format="BGR", size=None):
+    """Starts the upload (FrameUploader.prefetch) of the host frame a later device_frame call will get; a device frame
+    needs none."""
+    f = as_frame(frame, pixel_format, size)
+    if not f.on_device:
+        uploader.prefetch(f.y)

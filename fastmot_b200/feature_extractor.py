@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import _lib, models
-from .devmem import ptr, stream_ptr, FrameUploader, Frame, nv12_frame
+from .devmem import ptr, stream_ptr, device_frame, UploadSlot
 from .tracker import DeviceEmbeddings
 
 
@@ -32,7 +32,7 @@ class FeatureExtractor:
         dev = torch.device("cuda")
         self._tlbr_dev = torch.zeros(max_crops, 4, dtype=torch.float64, device=dev)
         self._tlbr_host = torch.zeros(max_crops, 4, dtype=torch.float64).pin_memory()
-        self._uploader = None
+        self._upload = UploadSlot()
         self.last_num_features = 0
         self._out = None
         self._splits = None         # per-stream crop offsets of the last extract_multi_async
@@ -70,32 +70,14 @@ class FeatureExtractor:
             return
         if n > self.max_crops:
             raise MemoryError(f"{n} crops > max_crops {self.max_crops}")
-        if isinstance(frame, Frame) and frame.format == "BGR":
-            frame = frame.y
-        fmt = frame.format if isinstance(frame, Frame) else "BGR"
-        if torch.is_tensor(frame) or (isinstance(frame, Frame) and frame.on_device):
-            frame_dev = frame
-        else:
-            w, h = frame.size if isinstance(frame, Frame) else (frame.shape[1], frame.shape[0])
-            if self._uploader is None or self._uploader.pixel_format != fmt or \
-                    self._uploader.shape != FrameUploader.frame_shape((w, h), fmt):
-                self._uploader = FrameUploader((w, h), pixel_format=fmt)
-            frame_dev = self._uploader.upload(frame.y if fmt == "NV12" else frame)
-            frame_dev = nv12_frame(frame_dev) if fmt == "NV12" else frame_dev
+        frame_dev = device_frame(frame, self._upload)
         eng = self._engine(n)
         self._tlbr_host[:n] = torch.as_tensor(tlbrs)
         self._tlbr_dev[:n].copy_(self._tlbr_host[:n], non_blocking=True)
         c, ih, iw = self.model.INPUT_SHAPE
-        if fmt == "NV12":
-            rc = self._lib.fm_roi_resize_norm_nv12(*frame_dev.nv12_args(), frame_dev.w, frame_dev.h,
-                                                   ptr(self._tlbr_dev), None, n, iw, ih, eng.inp_layout, ptr(eng.inp),
-                                                   stream_ptr())
-            _lib.check(rc, "fm_roi_resize_norm_nv12")
-        else:
-            h, w = frame_dev.shape[:2]
-            rc = self._lib.fm_roi_resize_norm(ptr(frame_dev), w, h, ptr(self._tlbr_dev), None, n, iw, ih,
-                                              eng.inp_layout, ptr(eng.inp), stream_ptr())
-            _lib.check(rc, "fm_roi_resize_norm")
+        rc = self._lib.fm_roi_resize_norm(C.byref(frame_dev.fm()), ptr(self._tlbr_dev), None, n, iw, ih, eng.inp_layout,
+                                          ptr(eng.inp), stream_ptr())
+        _lib.check(rc, "fm_roi_resize_norm")
         self._out = eng.forward(n)
 
     def extract_multi_async(self, frames, tlbrs_per_stream):
@@ -118,9 +100,7 @@ class FeatureExtractor:
             raise MemoryError(f"{n} crops > max_crops {self.max_crops}")
         rows = (_lib.FmFrameGeom * len(frames))()
         for r, f in zip(rows, frames):
-            if not (isinstance(f, Frame) and f.on_device):
-                f = Frame.bgr(f)
-            f.fill_geom(r)
+            r.frame = device_frame(f).fm()
         nb = C.sizeof(rows)
         if self._geom_host is None or self._geom_host.numel() < nb:
             if self._geom_ev is not None:

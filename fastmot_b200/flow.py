@@ -16,7 +16,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .devmem import ptr, stream_ptr, FrameUploader, Frame, nv12_frame
+from .devmem import ptr, stream_ptr, device_frame, UploadSlot, FrameUploader
 
 LOGGER = logging.getLogger(__name__)
 
@@ -167,8 +167,7 @@ class Flow:
         self.rounds_last = 0
         self._affine_args = (0, size[0], size[1])
         self._h_slots = torch.zeros(max_tracks, dtype=i32).pin_memory()
-        self._uploader = FrameUploader(size)
-        self._nv12_uploader = None
+        self._upload = UploadSlot(FrameUploader(size))
         self._side = torch.cuda.Stream()
         self._ev_lk = torch.cuda.Event()
         self._ev_h = torch.cuda.Event()
@@ -274,38 +273,21 @@ class Flow:
 
     # ------------------------------------------------------------------
     def _to_device(self, frame):
-        """BGR frames: the cuda tensor, or the uploaded host array.  A Frame (any format) of this stage's size: the
-        device Frame, host NV12 frames uploaded."""
-        if isinstance(frame, Frame):
-            if frame.size != tuple(self.size):
-                raise ValueError(f"frame of size {frame.size}, the optical-flow stage's is {tuple(self.size)}")
-            if frame.format == "BGR" or frame.on_device:
-                return frame.y if frame.format == "BGR" else frame
-            if self._nv12_uploader is None:
-                self._nv12_uploader = FrameUploader(self.size, pixel_format="NV12")
-            return nv12_frame(self._nv12_uploader.upload(frame.y))
-        return frame if torch.is_tensor(frame) else self._uploader.upload(frame)
+        """The device Frame of a frame of this stage's size (BGR, or an NV12 Frame); host frames are uploaded."""
+        return device_frame(frame, self._upload, size=self.size)
 
     def _preprocess(self, frame_dev, k):
-        """cvtColor + resize (flow.py:153-154) and the LK pyramid with derivatives for buffer k."""
-        W, H = self.size
+        """cvtColor + resize (flow.py:153-154) and the LK pyramid with derivatives for buffer k (frame_dev: a device
+        Frame or an HxWx3 u8 cuda tensor of this stage's size)."""
         s = stream_ptr()
         lib = self._lib
-        if isinstance(frame_dev, Frame):                     # NV12, read in place
-            if self._half:
-                _lib.check(lib.fm_gray_half_nv12(*frame_dev.nv12_args(), W, H, ptr(self.gray[k]),
-                                                 ptr(self.pyr[k][0]), s), "fm_gray_half_nv12")
-            else:
-                sw, sh = self.opt_flow_sz
-                _lib.check(lib.fm_gray_resize_nv12(*frame_dev.nv12_args(), W, H, ptr(self.gray[k]),
-                                                   ptr(self.pyr[k][0]), sw, sh, s), "fm_gray_resize_nv12")
-        elif self._half:
-            _lib.check(lib.fm_gray_half(ptr(frame_dev), W, H, ptr(self.gray[k]), ptr(self.pyr[k][0]), s),
-                       "fm_gray_half")
+        frame_dev = device_frame(frame_dev, size=self.size)
+        fm = C.byref(frame_dev.fm())
+        if self._half:
+            _lib.check(lib.fm_gray_half(fm, ptr(self.gray[k]), ptr(self.pyr[k][0]), s), "fm_gray_half")
         else:
             sw, sh = self.opt_flow_sz
-            _lib.check(lib.fm_gray_resize(ptr(frame_dev), W, H, ptr(self.gray[k]), ptr(self.pyr[k][0]), sw, sh, s),
-                       "fm_gray_resize")
+            _lib.check(lib.fm_gray_resize(fm, ptr(self.gray[k]), ptr(self.pyr[k][0]), sw, sh, s), "fm_gray_resize")
         for i, (w, h) in enumerate(self.level_sizes):
             if i + 1 < len(self.level_sizes):
                 _lib.check(lib.fm_pyr_level(ptr(self.pyr[k][i]), w, h, ptr(self.pyr[k][i + 1]), s), "fm_pyr_level")
@@ -341,14 +323,9 @@ class Flow:
         runner = self._get_runner()
         if runner is not None:
             main = torch.cuda.current_stream()
-            if isinstance(frame_dev, Frame):
-                _lib.check(lib.fm_flow_predict_nv12(runner, *frame_dev.nv12_args(), self.prev, n, ptr(h_dev),
-                                                    ptr(h_ok_dev), C.c_void_p(main.cuda_stream),
-                                                    C.c_void_p(self._side.cuda_stream)), "fm_flow_predict_nv12")
-            else:
-                _lib.check(lib.fm_flow_predict(runner, ptr(frame_dev), self.prev, n, ptr(h_dev), ptr(h_ok_dev),
-                                               C.c_void_p(main.cuda_stream), C.c_void_p(self._side.cuda_stream)),
-                           "fm_flow_predict")
+            _lib.check(lib.fm_flow_predict(runner, C.byref(frame_dev.fm()), self.prev, n, ptr(h_dev), ptr(h_ok_dev),
+                                           C.c_void_p(main.cuda_stream), C.c_void_p(self._side.cuda_stream)),
+                       "fm_flow_predict")
             self.prev = cur                      # flow.py:212-213
             self._bg_cache = None
             self._affine_args = (n, W, H)

@@ -16,7 +16,7 @@ import torch
 from .detector import YOLODetector, PublicDetector
 from .feature_extractor import FeatureExtractor
 from .tracker import MultiTracker
-from .devmem import FrameUploader, check_pixel_format, device_frame, nv12_frame
+from .devmem import FrameUploader, check_pixel_format, device_frame, prefetch_frame
 from .utils import Profiler
 
 LOGGER = logging.getLogger(__name__)
@@ -128,16 +128,11 @@ class MOT:
         """Optional read-ahead: starts the host-to-device copy of the NEXT frame (the ndarray a later `step` call will
         receive) on an upload stream, so it overlaps the current step's kernels (role of the reference's VideoIO
         frame queue, fastmot/videoio.py:125-142)."""
-        if self.pixel_format == 'NV12':
-            f = nv12_frame(frame)
-            if not f.on_device:
-                self._uploader.prefetch(f.y)
-        elif not torch.is_tensor(frame):
-            self._uploader.prefetch(frame)
+        prefetch_frame(frame, self._uploader, self.pixel_format, self.size)
 
     def step(self, frame):
         """mot.py:125-168"""
-        frame_dev = device_frame(frame, self.pixel_format, self._uploader)
+        frame_dev = device_frame(frame, self._uploader, self.pixel_format, self.size)
         detections = []
         if self.frame_count == 0:
             self._detect_async(frame_dev)

@@ -21,7 +21,7 @@ import torch
 from .detector import YOLODetector
 from .feature_extractor import FeatureExtractor
 from .tracker import MultiTracker
-from .devmem import FrameUploader, check_pixel_format, device_frame, nv12_frame
+from .devmem import FrameUploader, check_pixel_format, device_frame, prefetch_frame
 from .mot import DetectorType
 from .utils import Profiler
 
@@ -131,28 +131,20 @@ class MultiCameraMOT:
 
     def prefetch(self, frames):
         """Starts the uploads of the frames a later `step` call will receive (host arrays only; None is skipped)."""
-        self._check_frames(frames)
-        for up, f in zip(self._uploaders, frames):
-            if f is None:
-                continue
-            if self.pixel_format == 'NV12':
-                f = nv12_frame(f)
-                if not f.on_device:
-                    up.prefetch(f.y)
-            elif not torch.is_tensor(f):
-                up.prefetch(f)
+        self._each_frame(prefetch_frame, frames)
 
-    def _check_frames(self, frames):
+    def _each_frame(self, fn, frames):
+        """[fn(frame, camera's uploader, pixel format, camera's size) or None] over the cameras' frames (None: no
+        frame); a frame of the wrong size or form raises ValueError naming its camera."""
         if len(frames) != self.num_cameras:
             raise ValueError(f"expected {self.num_cameras} frames, got {len(frames)}")
-        for s, (f, (w, h)) in enumerate(zip(frames, self.sizes)):
-            if f is None:
-                continue
-            if self.pixel_format == 'NV12':
-                if nv12_frame(f).size != (w, h):
-                    raise ValueError(f"camera {s}: NV12 frame of size {nv12_frame(f).size}, expected {(w, h)}")
-            elif tuple(f.shape) != (h, w, 3):
-                raise ValueError(f"camera {s}: frame of shape {tuple(f.shape)}, expected {(h, w, 3)}")
+        out = []
+        for s, (f, up, wh) in enumerate(zip(frames, self._uploaders, self.sizes)):
+            try:
+                out.append(None if f is None else fn(f, up, self.pixel_format, wh))
+            except ValueError as e:
+                raise ValueError(f"camera {s}: {e}") from None
+        return out
 
     def _detect_async(self, frames_dev):
         self._main_ready.record()
@@ -169,9 +161,7 @@ class MultiCameraMOT:
     def step(self, frames):
         """One step of the group: frames[s] is camera s's next frame in the group's pixel format (HxWx3 u8 host array
         or cuda tensor; NV12 in any form MOT takes), or None when camera s has no frame on this step."""
-        self._check_frames(frames)
-        frames_dev = [None if f is None else device_frame(f, self.pixel_format, up)
-                      for f, up in zip(frames, self._uploaders)]
+        frames_dev = self._each_frame(device_frame, frames)
         init, detect, track = plan_step(self.frame_counts, [f is not None for f in frames], self.detector_frame_skip)
         cams = sorted(init + detect)                 # the detector batch, in camera order
         if not cams:

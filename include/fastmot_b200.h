@@ -165,60 +165,59 @@ typedef struct FmYoloHead {
 
 /* Pixel formats of the frames the letterbox, crop and KLT gray kernels read.  NV12 (what hardware video decoders
  * emit): a Y plane of h rows and a UV plane of h / 2 rows, both w bytes wide (U, V interleaved at half resolution),
- * each with its own row pitch in bytes (>= w), w and h even.  Every *_nv12 entry point gives bit for bit what its BGR
- * entry gives on cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12) (OpenCV 4.13: BT.601 limited range, 20-bit fixed point,
+ * each with its own row pitch in bytes, w and h even.  Every entry gives on an NV12 frame bit for bit what it gives on
+ * the BGR frame cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12) (OpenCV 4.13: BT.601 limited range, 20-bit fixed point,
  * nearest-neighbour chroma); the pixels are converted inline, no BGR frame is written. */
 #define FM_PIX_BGR 0
 #define FM_PIX_NV12 1
 
-/* One frame of a batch whose frames may differ in size: the device frame (BGR u8 HWC, w x h), its letterbox ROI in the
- * network input, and the pixel scale (size_w, size_h = upscaled_sz) and offset (off_x, off_y = bbox_offset) the head
- * decode maps its boxes back with -- the values a one-frame detector of that size passes as scalars.  The pixel-format
- * fields come last, so a row whose tail is zero is a tight BGR frame; an FM_PIX_NV12 row has its Y plane in `frame`,
- * its UV plane in `uv` and their row pitches in `pitch` / `uv_pitch` (0 = w). */
-typedef struct FmFrameGeom {
-    const unsigned char* frame;
-    int w, h;
-    int roi_x, roi_y, roi_w, roi_h;
-    float size_w, size_h, off_x, off_y;
+/* One camera frame in device memory, as every entry that reads camera pixels takes it.
+ *   FM_PIX_BGR : y is the tight u8 HWC frame (w * 3 bytes per row); uv, pitch and uv_pitch are ignored.
+ *   FM_PIX_NV12: y and uv are the two planes, pitch and uv_pitch their row pitches in bytes (0 = w, else >= w).
+ * The one-frame entries take a host pointer to it and reject a NULL y, an empty frame, an unknown format and an NV12
+ * frame that breaks the rules above. */
+typedef struct FmFrame {
+    const unsigned char* y;
     const unsigned char* uv;
+    int w, h;
     int pitch, uv_pitch;
     int format;
+} FmFrame;
+
+/* One frame of a batch whose frames may differ in size: the device frame, its letterbox ROI in the network input, and
+ * the pixel scale (size_w, size_h = upscaled_sz) and offset (off_x, off_y = bbox_offset) the head decode maps its boxes
+ * back with -- the values a one-frame detector of that size passes as scalars. */
+typedef struct FmFrameGeom {
+    FmFrame frame;
+    int roi_x, roi_y, roi_w, roi_h;
+    float size_w, size_h, off_x, off_y;
 } FmFrameGeom;
 
-/* YOLODetector._preprocess + _create_letterbox (fastmot/detector.py:289-320): bilinear resize of the BGR u8 HWC
- * frame into the ROI [roi_x, roi_y, roi_w, roi_h] of a dst_w x dst_h network input (half-pixel centres, edge
- * replicate, rounded to u8 like the reference's CuPy zoom), BGR->RGB, x/255; everything outside the ROI = 0.5.
+/* YOLODetector._preprocess + _create_letterbox (fastmot/detector.py:289-320): bilinear resize of the frame into the
+ * ROI [roi_x, roi_y, roi_w, roi_h] of a dst_w x dst_h network input (half-pixel centres, edge replicate, rounded to u8
+ * like the reference's CuPy zoom), BGR->RGB, x/255; everything outside the ROI = 0.5.  An NV12 frame's four bilinear
+ * taps are each converted to BGR with their own chroma sample before they are interpolated.
  * layout 0: fp32 planar CHW (the reference's TensorRT input); layout 1: fp16 NHWC, C padded to 8 (16 bytes per pixel). */
-int fm_letterbox_preproc(const unsigned char* frame, int src_w, int src_h, int dst_w, int dst_h, int roi_x, int roi_y,
-                         int roi_w, int roi_h, int layout, void* out, void* stream);
-/* fm_letterbox_preproc of an NV12 frame (y / uv planes, row pitches in bytes; see FM_PIX_NV12): each of the four
- * bilinear taps is converted to BGR with its own chroma sample before it is interpolated. */
-int fm_letterbox_preproc_nv12(const unsigned char* y, const unsigned char* uv, int y_pitch, int uv_pitch, int src_w,
-                              int src_h, int dst_w, int dst_h, int roi_x, int roi_y, int roi_w, int roi_h, int layout,
-                              void* out, void* stream);
+int fm_letterbox_preproc(const FmFrame* frame, int dst_w, int dst_h, int roi_x, int roi_y, int roi_w, int roi_h,
+                         int layout, void* out, void* stream);
 /* fm_letterbox_preproc (layout 1) of `batch` frames of any sizes and formats in one launch: geom is a DEVICE array of
- * batch rows (frame, w, h, roi_* and the format fields are read; every roi_w, roi_h > 0); out is fp16
- * [batch][dst_h][dst_w][8], image b bit-identical to the one-frame call (BGR or _nv12) on geom[b]'s frame, size and
- * ROI. */
+ * batch rows (frame and roi_* are read; every roi_w, roi_h > 0); out is fp16 [batch][dst_h][dst_w][8], image b
+ * bit-identical to the one-frame call on geom[b]'s frame and ROI. */
 int fm_letterbox_preproc_geom(const FmFrameGeom* geom, int batch, int dst_w, int dst_h, void* out, void* stream);
 
 /* FeatureExtractor.extract_async preprocessing (fastmot/feature_extractor.py:48-60, 84-98; rect.py:92-97) for all
  * crops in one launch: integer-truncated clamp crop, OpenCV INTER_LINEAR 8-bit fixed-point resize to
- * out_w x out_h, BGR->RGB, (x/255 - mean)/std.  n = min(*n_dev, n_max) if n_dev != NULL else n_max.
+ * out_w x out_h, BGR->RGB, (x/255 - mean)/std (an NV12 frame's taps are converted to BGR before they are
+ * interpolated).  n = min(*n_dev, n_max) if n_dev != NULL else n_max.
  * layout as above; output is [n][3][out_h][out_w] f32 or [n][out_h][out_w][8] f16; layout 2: fp16
  * [n][out_h + 8][out_w + 8][4] with the crop at (+4, +4) inside a border the CALLER zeroed once (the zero padding of
  * the OSNet 7x7 stem, fm_osnet_stem). */
-int fm_roi_resize_norm(const unsigned char* frame, int src_w, int src_h, const double* tlbrs, const int* n_dev,
-                       int n_max, int out_w, int out_h, int layout, void* out, void* stream);
-/* fm_roi_resize_norm of an NV12 frame (see FM_PIX_NV12); each tap is converted to BGR before it is interpolated. */
-int fm_roi_resize_norm_nv12(const unsigned char* y, const unsigned char* uv, int y_pitch, int uv_pitch, int src_w,
-                            int src_h, const double* tlbrs, const int* n_dev, int n_max, int out_w, int out_h,
-                            int layout, void* out, void* stream);
+int fm_roi_resize_norm(const FmFrame* frame, const double* tlbrs, const int* n_dev, int n_max, int out_w, int out_h,
+                       int layout, void* out, void* stream);
 /* fm_roi_resize_norm over several frames of any sizes and formats in one launch: crop i (tlbrs[i]) is cut from
- * geom[frame_idx[i]]'s frame, clamped to and addressed with that row's w and h (geom: DEVICE FmFrameGeom array, the ROI
- * and scale fields are not read; frame_idx: device int32 [n]); each crop is bit-identical to the one-frame call (BGR or
- * _nv12) on its own frame and box. */
+ * geom[frame_idx[i]]'s frame, clamped to and addressed with that frame's w and h (geom: DEVICE FmFrameGeom array, the
+ * ROI and scale fields are not read; frame_idx: device int32 [n]); each crop is bit-identical to the one-frame call on
+ * its own frame and box. */
 int fm_roi_resize_norm_geom(const FmFrameGeom* geom, const int* frame_idx, const double* tlbrs, int n, int out_w,
                             int out_h, int layout, void* out, void* stream);
 
@@ -350,18 +349,12 @@ typedef struct FmTrackJob {      /* per-track record produced by fm_flow_keypoin
     int pad;
 } FmTrackJob;
 
-/* cv2.cvtColor(BGR2GRAY) + cv2.resize(0.5x) of flow.py:153-154 / :129-131 in one pass (w, h even). */
-int fm_gray_half(const unsigned char* frame, int w, int h, unsigned char* gray, unsigned char* small, void* stream);
+/* cv2.cvtColor(BGR2GRAY) + cv2.resize(0.5x) of flow.py:153-154 / :129-131 in one pass (w, h even); gray is
+ * frame->w x h.  On an NV12 frame a thread's 2x2 block is one chroma sample (one UV load). */
+int fm_gray_half(const FmFrame* frame, unsigned char* gray, unsigned char* small, void* stream);
 /* cv2.cvtColor(BGR2GRAY) + cv2.resize(gray, (sw, sh)) INTER_LINEAR at any optical-flow size 0 < sw <= w,
  * 0 < sh <= h (odd frame sizes, anisotropic scales, scale 1). */
-int fm_gray_resize(const unsigned char* frame, int w, int h, unsigned char* gray, unsigned char* small, int sw, int sh,
-                   void* stream);
-/* fm_gray_half / fm_gray_resize of an NV12 frame (see FM_PIX_NV12): the gray value of BGR = cvtColor(NV12 -> BGR); in
- * fm_gray_half a thread's 2x2 block is one chroma sample (one UV load). */
-int fm_gray_half_nv12(const unsigned char* y, const unsigned char* uv, int y_pitch, int uv_pitch, int w, int h,
-                      unsigned char* gray, unsigned char* small, void* stream);
-int fm_gray_resize_nv12(const unsigned char* y, const unsigned char* uv, int y_pitch, int uv_pitch, int w, int h,
-                        unsigned char* gray, unsigned char* small, int sw, int sh, void* stream);
+int fm_gray_resize(const FmFrame* frame, unsigned char* gray, unsigned char* small, int sw, int sh, void* stream);
 /* one pyrDown step ((sw+1)/2 x (sh+1)/2) and the Scharr derivative image of a level — what
  * cv2.calcOpticalFlowPyrLK builds internally (flow.py:203-207). */
 int fm_pyr_level(const unsigned char* src, int sw, int sh, unsigned char* dst, void* stream);
@@ -497,15 +490,9 @@ typedef struct FmFlowPlan {
 } FmFlowPlan;
 void* fm_flow_plan_create(const FmFlowPlan* plan);      /* NULL on error (fm_last_error) */
 void fm_flow_plan_destroy(void* handle);
-/* flow.py:121-133 / :153-154 for buffer k (0 / 1) */
-int fm_flow_preprocess(void* handle, const unsigned char* frame, int k, void* stream);
-int fm_flow_predict(void* handle, const unsigned char* frame, int prev, int n_trk, double* H_out, int* h_ok,
-                    void* s_main, void* s_side);
-/* the same two calls on an NV12 frame (planes and row pitches as in FM_PIX_NV12; the plan's frame_w x frame_h even) */
-int fm_flow_preprocess_nv12(void* handle, const unsigned char* y, const unsigned char* uv, int y_pitch, int uv_pitch,
-                            int k, void* stream);
-int fm_flow_predict_nv12(void* handle, const unsigned char* y, const unsigned char* uv, int y_pitch, int uv_pitch,
-                         int prev, int n_trk, double* H_out, int* h_ok, void* s_main, void* s_side);
+/* frame: the plan's frame_w x frame_h (anything else is rejected) */
+int fm_flow_predict(void* handle, const FmFrame* frame, int prev, int n_trk, double* H_out, int* h_ok, void* s_main,
+                    void* s_side);
 
 /* ---------------------------------------------------------------- tensor-core primitive self-test ----------- */
 /* One CTA exercises the building blocks of the fused kernels (csrc/tc_common.cuh): TMA tensor-map load of a

@@ -14,10 +14,11 @@ consumes it (one copy per frame).  A run is `warmup` steps, then `steps` steps t
 stream.  `h2d_frame_bytes` is counted from the frame copies MOT's uploader made in the timed steps.
 
 Kernel times: CUDA events around `kernel-reps` back-to-back launches of the one-frame entry points on a 1080p frame
-(letterbox into the csp-640 input, 200 crops into the OSNet input layout, gray + 0.5x image), BGR and NV12, median of
-five sets.  Prints the card name and power limit, then one JSON line.
+(letterbox into the csp-640 input, 200 crops into the OSNet input layout, gray + 0.5x image), each on a BGR and an NV12
+FmFrame, median of five sets.  Prints the card name and power limit, then one JSON line.
 """
 import argparse
+import ctypes as C
 import json
 import os
 import sys
@@ -93,7 +94,7 @@ def kernel_us(fn, reps):
     return round(float(np.median(out)), 2)
 
 
-def kernel_times(mot_bgr, bgr_dev, nv_frame, scene, reps):
+def kernel_times(mot_bgr, bgr_frame, nv_frame, scene, reps):
     from fastmot_b200 import _lib
     from fastmot_b200.devmem import ptr, stream_ptr
     lib = _lib.load()
@@ -109,23 +110,19 @@ def kernel_times(mot_bgr, bgr_dev, nv_frame, scene, reps):
     n = len(tl)
     gray = torch.empty(H, W, dtype=torch.uint8, device="cuda")
     small = torch.empty(H // 2, W // 2, dtype=torch.uint8, device="cuda")
-    nv = nv_frame.nv12_args()
     s = stream_ptr()
     calls = {
-        "letterbox": (lambda: lib.fm_letterbox_preproc(ptr(bgr_dev), W, H, in_w, in_h, rx, ry, rw, rh, 1, ptr(inp), s),
-                      lambda: lib.fm_letterbox_preproc_nv12(*nv, W, H, in_w, in_h, rx, ry, rw, rh, 1, ptr(inp), s)),
-        "crops": (lambda: lib.fm_roi_resize_norm(ptr(bgr_dev), W, H, ptr(tl), None, n, iw, ih, eng.inp_layout,
-                                                 ptr(crops), s),
-                  lambda: lib.fm_roi_resize_norm_nv12(*nv, W, H, ptr(tl), None, n, iw, ih, eng.inp_layout, ptr(crops),
-                                                      s)),
-        "gray_half": (lambda: lib.fm_gray_half(ptr(bgr_dev), W, H, ptr(gray), ptr(small), s),
-                      lambda: lib.fm_gray_half_nv12(*nv, W, H, ptr(gray), ptr(small), s)),
+        "letterbox": lambda f: lib.fm_letterbox_preproc(f, in_w, in_h, rx, ry, rw, rh, 1, ptr(inp), s),
+        "crops": lambda f: lib.fm_roi_resize_norm(f, ptr(tl), None, n, iw, ih, eng.inp_layout, ptr(crops), s),
+        "gray_half": lambda f: lib.fm_gray_half(f, ptr(gray), ptr(small), s),
     }
+    frames = {"bgr_us": C.byref(bgr_frame.fm()), "nv12_us": C.byref(nv_frame.fm())}
     out = {}
-    for name, (fb, fn) in calls.items():
-        _lib.check(fb(), name)
-        _lib.check(fn(), name + "_nv12")
-        out[name] = {"bgr_us": kernel_us(fb, reps), "nv12_us": kernel_us(fn, reps)}
+    for name, call in calls.items():
+        out[name] = {}
+        for key, f in frames.items():
+            _lib.check(call(f), f"{name} {key}")
+            out[name][key] = kernel_us(lambda: call(f), reps)
     out["crops"]["n"] = n
     return out
 
@@ -141,7 +138,7 @@ def main():
     import bench
     from bench_multistream import card
     from fastmot_b200 import _lib
-    from fastmot_b200.devmem import nv12_frame
+    from fastmot_b200.devmem import Frame, nv12_frame
     from oracle.nv12 import bgr_to_nv12
     _lib.require_device()
     print(json.dumps(card()), flush=True)
@@ -174,8 +171,8 @@ def main():
                  for (fmt, where), v in runs.items()},
         "tracks_equal": all(t == ref for t in tracks.values()),
         "visible_tracks": len(ref),
-        "kernels": kernel_times(mots["BGR"], frames[("BGR", "device")][0], nv12_frame(frames[("NV12", "device")][0]),
-                                scene, args.kernel_reps),
+        "kernels": kernel_times(mots["BGR"], Frame.bgr(frames[("BGR", "device")][0]),
+                                nv12_frame(frames[("NV12", "device")][0]), scene, args.kernel_reps),
     }
     print(json.dumps(out), flush=True)
 

@@ -1,6 +1,7 @@
 """GPU parity: detector pre/post-processing kernels (csrc/preproc.cu, csrc/detect.cu) vs the reference golden
 and the oracle.  Box/label lists bit-exact for new_coords heads and for the NMS stage; old-coords heads use
 __expf so boxes may move by <= 1 px at rounding boundaries."""
+import ctypes as C
 import os
 
 import numpy as np
@@ -133,9 +134,9 @@ def test_empty_detections():
 
 
 @pytest.mark.parametrize("model_name", ["YOLOv4CSP", "YOLOv4Tiny"])
-def test_letterbox_preproc(model_name):
+def test_letterbox_preproc_fmframe(model_name):
     from fastmot_b200 import _lib, models
-    from fastmot_b200.devmem import ptr, stream_ptr
+    from fastmot_b200.devmem import Frame, ptr, stream_ptr
     from fastmot_b200.synth import SyntheticScene
     from oracle import detect
     lib = _lib.load()
@@ -144,23 +145,24 @@ def test_letterbox_preproc(model_name):
     frame = SyntheticScene(30, seed=2).frame(1)
     roi, _, _ = detect.letterbox_geometry((1920, 1080), (W, H), model.LETTERBOX)
     want = detect.letterbox(frame, (W, H), roi)
-    fd = torch.as_tensor(frame).to("cuda")
+    fr = Frame.bgr(torch.as_tensor(frame).to("cuda"))
+    fd = C.byref(fr.fm())
     out32 = torch.zeros(3, H, W, dtype=torch.float32, device="cuda")
-    _lib.check(lib.fm_letterbox_preproc(ptr(fd), 1920, 1080, W, H, *roi, 0, ptr(out32), stream_ptr()), "lb")
+    _lib.check(lib.fm_letterbox_preproc(fd, W, H, *roi, 0, ptr(out32), stream_ptr()), "lb")
     got = out32.cpu().numpy()
     diff = np.abs(got - want) * 255
     assert diff.max() <= 1.0 + 1e-3            # reference semantics pinned only to +-1 LSB (CuPy absent)
     assert (diff < 1e-3).mean() > 0.999
     out16 = torch.zeros(H, W, 8, dtype=torch.float16, device="cuda")
-    _lib.check(lib.fm_letterbox_preproc(ptr(fd), 1920, 1080, W, H, *roi, 1, ptr(out16), stream_ptr()), "lb")
+    _lib.check(lib.fm_letterbox_preproc(fd, W, H, *roi, 1, ptr(out16), stream_ptr()), "lb")
     g16 = out16.cpu().float().numpy()
     assert np.abs(g16[..., :3].transpose(2, 0, 1) - got).max() <= 1e-3
     assert np.all(g16[..., 3:] == 0)
 
 
-def test_roi_resize_norm():
+def test_roi_resize_norm_fmframe():
     from fastmot_b200 import _lib
-    from fastmot_b200.devmem import ptr, stream_ptr
+    from fastmot_b200.devmem import Frame, ptr, stream_ptr
     from fastmot_b200.synth import SyntheticScene
     from oracle import detect
     lib = _lib.load()
@@ -169,13 +171,13 @@ def test_roi_resize_norm():
     tl = sc.detections(0)[0]
     tl = np.concatenate([tl, [[-5.5, 10.2, 40.7, 90.9], [1890, 1000, 1950, 1100], [100, 100, 400, 700]]])
     want = detect.roi_preprocess(frame, tl)                  # cv2.resize path of the reference
-    fd = torch.as_tensor(frame).to("cuda")
+    fr = Frame.bgr(torch.as_tensor(frame).to("cuda"))
+    fd = C.byref(fr.fm())
     td = torch.as_tensor(np.ascontiguousarray(tl, np.float64)).to("cuda")
     n = len(tl)
     out = torch.zeros(n, 3, 256, 128, dtype=torch.float32, device="cuda")
     ncnt = torch.tensor([n], dtype=torch.int32, device="cuda")
-    _lib.check(lib.fm_roi_resize_norm(ptr(fd), 1920, 1080, ptr(td), ptr(ncnt), n + 5, 128, 256, 0, ptr(out),
-                                      stream_ptr()), "roi")
+    _lib.check(lib.fm_roi_resize_norm(fd, ptr(td), ptr(ncnt), n + 5, 128, 256, 0, ptr(out), stream_ptr()), "roi")
     got = out.cpu().numpy()
     std = np.array([0.229, 0.224, 0.225])[None, :, None, None]
     lsb = np.abs(got - want) * 255 * std
@@ -184,7 +186,6 @@ def test_roi_resize_norm():
     exact = detect.roi_preprocess_fixedpoint(frame, tl)      # the formula the kernel implements
     np.testing.assert_allclose(got, exact, atol=2e-6)
     out16 = torch.zeros(n, 256, 128, 8, dtype=torch.float16, device="cuda")
-    _lib.check(lib.fm_roi_resize_norm(ptr(fd), 1920, 1080, ptr(td), None, n, 128, 256, 1, ptr(out16),
-                                      stream_ptr()), "roi")
+    _lib.check(lib.fm_roi_resize_norm(fd, ptr(td), None, n, 128, 256, 1, ptr(out16), stream_ptr()), "roi")
     g16 = out16.cpu().float().numpy()[..., :3].transpose(0, 3, 1, 2)
     assert np.abs(g16 - got).max() <= 2e-3

@@ -8,6 +8,7 @@ kernels under it, on YOLOv4-tiny (no letterbox) and YOLOv4-csp (letterbox; the 4
 - A batch-3 engine sharing a batch-4 engine's memory passes the launch-by-launch float64 check, leaves the 4th image
   alone, gives the heads of a standalone batch-3 engine and allocates (almost) nothing.
 """
+import ctypes as C
 import time
 from types import SimpleNamespace as NS
 
@@ -160,9 +161,9 @@ def gcase(request):
     c.close()
 
 
-def test_geom_letterbox_equals_one_frame_letterbox(gcase):
+def test_geom_letterbox_equals_fmframe_letterbox(gcase):
     from fastmot_b200 import _lib
-    from fastmot_b200.devmem import ptr, stream_ptr
+    from fastmot_b200.devmem import Frame, ptr, stream_ptr
     det = gcase.det
     lib = _lib.load()
     rois = [det.geometry(wh)[0] for wh in SIZES]
@@ -171,8 +172,10 @@ def test_geom_letterbox_equals_one_frame_letterbox(gcase):
     for b, (f, wh) in enumerate(zip(gcase.frames, SIZES)):
         rx, ry, rw, rh = rois[b]
         one = torch.zeros_like(det.inp[0])
-        _lib.check(lib.fm_letterbox_preproc(ptr(f), wh[0], wh[1], det.input_wh[0], det.input_wh[1], rx, ry, rw, rh, 1,
-                                            ptr(one), stream_ptr()), "fm_letterbox_preproc")
+        fm = Frame.bgr(f).fm()
+        assert (fm.w, fm.h) == wh
+        _lib.check(lib.fm_letterbox_preproc(C.byref(fm), det.input_wh[0], det.input_wh[1], rx, ry, rw, rh, 1, ptr(one),
+                                            stream_ptr()), "fm_letterbox_preproc")
         torch.cuda.synchronize()
         assert torch.equal(det.inp[b].view(torch.int16), one.view(torch.int16)), (gcase.name, b)
 
@@ -208,11 +211,11 @@ def test_geom_decode_and_nms_equal_one_image_path(gcase):
         assert np.array_equal(got[b].conf, want[2])
 
 
-def test_geom_crops_equal_one_frame_crops():
+def test_geom_crops_equal_fmframe_crops():
     """Mixed-size crops, including boxes past the right and bottom edges of the smaller frames, equal
     fm_roi_resize_norm on their own frame bit for bit."""
     from fastmot_b200 import _lib
-    from fastmot_b200.devmem import ptr, stream_ptr
+    from fastmot_b200.devmem import Frame, ptr, stream_ptr
     from fastmot_b200.feature_extractor import FeatureExtractor
     from fastmot_b200.synth import SyntheticScene
     lib = _lib.load()
@@ -234,8 +237,10 @@ def test_geom_crops_equal_one_frame_crops():
         n = len(boxes[s])
         one = torch.zeros_like(eng.inp[:n])
         tl = torch.as_tensor(boxes[s]).cuda()
-        _lib.check(lib.fm_roi_resize_norm(ptr(frames[s]), w, h, ptr(tl), None, n, 128, 256, eng.inp_layout,
-                                          ptr(one), stream_ptr()), "fm_roi_resize_norm")
+        fm = Frame.bgr(frames[s]).fm()
+        assert (fm.w, fm.h) == (w, h)
+        _lib.check(lib.fm_roi_resize_norm(C.byref(fm), ptr(tl), None, n, 128, 256, eng.inp_layout, ptr(one),
+                                          stream_ptr()), "fm_roi_resize_norm")
         torch.cuda.synchronize()
         assert torch.equal(eng.inp[r0:r0 + n].view(torch.int16), one.view(torch.int16)), s
         r0 += n
@@ -282,14 +287,14 @@ def test_shared_engine_launch_by_launch_heads_and_memory(gcase, monkeypatch):
 
 
 @pytest.mark.parametrize("name", MODELS)
-def test_frames_of_the_detectors_own_size_run_the_batch_b_engine(name, monkeypatch):
+def test_detector_size_frames_run_the_batch_b_engine(name, monkeypatch):
     """B = 2 different frames of the detector's own size through detect_batch_async: the batch-2 engine runs them (no
     batch-k engine is built), each image's letterbox equals fm_letterbox_preproc on its frame bit for bit, and each
     image's keys, candidate rows and detections equal the one-image decode + NMS of its head slice."""
     from test_gpu_yolo_zoo import _per_image_equals_one_image
     from fastmot_b200 import _lib
     from fastmot_b200.detector import YOLODetector
-    from fastmot_b200.devmem import ptr, stream_ptr
+    from fastmot_b200.devmem import Frame, ptr, stream_ptr
     from fastmot_b200.synth import SyntheticScene
     _synth_env(monkeypatch, name)
     size = SIZES[0]
@@ -302,8 +307,10 @@ def test_frames_of_the_detectors_own_size_run_the_batch_b_engine(name, monkeypat
     rx, ry, rw, rh = det.roi
     for b, f in enumerate(frames):
         one = torch.zeros_like(det.inp[0])
-        _lib.check(lib.fm_letterbox_preproc(ptr(f), size[0], size[1], det.input_wh[0], det.input_wh[1], rx, ry, rw, rh,
-                                            1, ptr(one), stream_ptr()), "fm_letterbox_preproc")
+        fm = Frame.bgr(f).fm()
+        assert (fm.w, fm.h) == tuple(size)
+        _lib.check(lib.fm_letterbox_preproc(C.byref(fm), det.input_wh[0], det.input_wh[1], rx, ry, rw, rh, 1, ptr(one),
+                                            stream_ptr()), "fm_letterbox_preproc")
         torch.cuda.synchronize()
         assert torch.equal(det.inp[b].view(torch.int16), one.view(torch.int16)), (name, b)
     assert not torch.equal(det.inp[0], det.inp[1])

@@ -8,6 +8,7 @@
 - Shared ReID batch: the multi-frame crops equal the one-frame crops bit for bit; the shared forward's per-stream
   embeddings agree with per-stream forwards, and its launches pass the float64 check at 3 x 67 crops.
 """
+import ctypes as C
 import os
 import time
 from types import SimpleNamespace as NS
@@ -157,16 +158,18 @@ def bcase(request):
     c.close()
 
 
-def test_batched_letterbox_equals_one_frame_letterbox(bcase):
+def test_batched_letterbox_equals_fmframe_letterbox(bcase):
     from fastmot_b200 import _lib
-    from fastmot_b200.devmem import ptr, stream_ptr
+    from fastmot_b200.devmem import Frame, ptr, stream_ptr
     det = bcase.det
     lib = _lib.load()
     rx, ry, rw, rh = det.roi
     for b, f in enumerate(bcase.frames):
         one = torch.zeros_like(det.inp[0])
-        _lib.check(lib.fm_letterbox_preproc(ptr(f), 1920, 1080, det.input_wh[0], det.input_wh[1], rx, ry, rw, rh, 1,
-                                            ptr(one), stream_ptr()), "fm_letterbox_preproc")
+        fm = Frame.bgr(f).fm()
+        assert (fm.w, fm.h) == (1920, 1080)
+        _lib.check(lib.fm_letterbox_preproc(C.byref(fm), det.input_wh[0], det.input_wh[1], rx, ry, rw, rh, 1, ptr(one),
+                                            stream_ptr()), "fm_letterbox_preproc")
         torch.cuda.synchronize()
         assert torch.equal(det.inp[b].view(torch.int16), one.view(torch.int16)), b
     assert not torch.equal(det.inp[0], det.inp[1])
@@ -350,13 +353,13 @@ def _boxes(n, seed):
     return np.stack([x0, y0, x0 + w, y0 + h], 1)
 
 
-def test_shared_reid_batch():
+def test_shared_reid_batch_equals_fmframe_crops():
     """3 streams x 67 crops (201, not a multiple of 8): every crop of fm_roi_resize_norm_geom equals the one-frame
     crop bit for bit; the shared forward's per-stream rows agree with one forward per stream (<= 5e-3 abs) and are
     views of the shared output; every launch of the shared forward passes the float64 check."""
     from test_gpu_osnet_ops import run_launch_by_launch
     from fastmot_b200 import _lib
-    from fastmot_b200.devmem import ptr, stream_ptr
+    from fastmot_b200.devmem import Frame, ptr, stream_ptr
     from fastmot_b200.feature_extractor import FeatureExtractor
     from fastmot_b200.synth import SyntheticScene
     from fastmot_b200.tracker import DeviceEmbeddings
@@ -374,8 +377,10 @@ def test_shared_reid_batch():
     for s in range(S):                                   # the crops, bit for bit
         one = torch.zeros_like(eng.inp[:n])
         tl = torch.as_tensor(boxes[s]).cuda()
-        _lib.check(lib.fm_roi_resize_norm(ptr(frames[s]), 1920, 1080, ptr(tl), None, n, 128, 256, eng.inp_layout,
-                                          ptr(one), stream_ptr()), "fm_roi_resize_norm")
+        fm = Frame.bgr(frames[s]).fm()
+        assert (fm.w, fm.h) == (1920, 1080)
+        _lib.check(lib.fm_roi_resize_norm(C.byref(fm), ptr(tl), None, n, 128, 256, eng.inp_layout, ptr(one),
+                                          stream_ptr()), "fm_roi_resize_norm")
         torch.cuda.synchronize()
         assert torch.equal(shared[s * n:(s + 1) * n].view(torch.int16), one.view(torch.int16)), s
     assert len(outs) == S and all(isinstance(o, DeviceEmbeddings) and len(o) == n for o in outs)

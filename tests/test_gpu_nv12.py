@@ -5,6 +5,7 @@ is always the BGR path fed cv2.cvtColor(nv12, cv2.COLOR_YUV2BGR_NV12); every com
 check runs on three device layouts of the same NV12 frame: tight (3H/2, W), pitched (row stride W + 64), and two planes
 in a padded-height decoder surface (Y in a surface of 1088 rows for 1080p, UV after it; padding filled with 255).
 """
+import ctypes as C
 from types import SimpleNamespace as NS
 
 import numpy as np
@@ -67,7 +68,7 @@ def _geom_table(frames, rois):
     from fastmot_b200 import _lib
     rows = (_lib.FmFrameGeom * len(frames))()
     for r, f, roi in zip(rows, frames, rois):
-        f.fill_geom(r)
+        r.frame = f.fm()
         r.roi_x, r.roi_y, r.roi_w, r.roi_h = roi
     return torch.frombuffer(bytearray(bytes(rows)), dtype=torch.uint8).cuda()
 
@@ -76,11 +77,11 @@ def _geom_table(frames, rois):
 @pytest.mark.parametrize("form", FORMS)
 @pytest.mark.parametrize("layout", [0, 1])
 @pytest.mark.parametrize("model", ["YOLOv4Tiny", "YOLOv4CSP"])
-def test_letterbox_nv12_equals_bgr_on_cv2_decode(model, layout, form):
+def test_letterbox_nv12_fmframe_equals_bgr_on_cv2_decode(model, layout, form):
     """Stretched (YOLOv4-tiny 416) and letterboxed (YOLOv4-csp 640) one-frame letterbox, fp32 CHW and fp16 NHWC8."""
     from fastmot_b200 import _lib, models
     from fastmot_b200.detector import letterbox_geometry
-    from fastmot_b200.devmem import ptr, stream_ptr
+    from fastmot_b200.devmem import Frame, ptr, stream_ptr
     lib = _lib.require_device()
     m = models.YOLO.get_model(model)
     _, in_h, in_w = m.INPUT_SHAPE
@@ -91,18 +92,18 @@ def test_letterbox_nv12_equals_bgr_on_cv2_decode(model, layout, form):
         want, got = (torch.full((3, in_h, in_w), -1.0, device="cuda") for _ in range(2))
     else:
         want, got = (torch.full((in_h, in_w, 8), -1.0, dtype=torch.float16, device="cuda") for _ in range(2))
-    bgr_dev = torch.as_tensor(bgr).cuda()
-    _lib.check(lib.fm_letterbox_preproc(ptr(bgr_dev), W, H, in_w, in_h, rx, ry, rw, rh, layout, ptr(want),
-                                        stream_ptr()), "fm_letterbox_preproc")
+    bgr_dev = Frame.bgr(torch.as_tensor(bgr).cuda())
+    _lib.check(lib.fm_letterbox_preproc(C.byref(bgr_dev.fm()), in_w, in_h, rx, ry, rw, rh, layout, ptr(want),
+                                        stream_ptr()), "fm_letterbox_preproc BGR")
     f = _frame(nv, form)
-    _lib.check(lib.fm_letterbox_preproc_nv12(*f.nv12_args(), W, H, in_w, in_h, rx, ry, rw, rh, layout, ptr(got),
-                                             stream_ptr()), "fm_letterbox_preproc_nv12")
+    _lib.check(lib.fm_letterbox_preproc(C.byref(f.fm()), in_w, in_h, rx, ry, rw, rh, layout, ptr(got), stream_ptr()),
+               "fm_letterbox_preproc NV12")
     assert _bits_equal(got, want)
     assert float(want.float().std()) > 0.05          # a real picture, not a constant
 
 
 @pytest.mark.parametrize("form", FORMS)
-def test_geometry_table_letterbox_and_crops_three_sizes(form):
+def test_geometry_table_fmframe_rows_three_sizes(form):
     """fm_letterbox_preproc_geom (YOLOv4-csp 640, each size its own ROI) and fm_roi_resize_norm_geom (layout 2) over
     1920x1080, 1280x720 and 1024x768 at once: an all-NV12 table and a mixed NV12 / BGR table give the all-BGR table's
     output on the cv2 decodes."""
@@ -140,10 +141,10 @@ def test_geometry_table_letterbox_and_crops_three_sizes(form):
 
 @pytest.mark.parametrize("form", FORMS)
 @pytest.mark.parametrize("layout", [0, 1, 2])
-def test_crops_nv12_equal_bgr_on_cv2_decode(layout, form):
+def test_crops_nv12_fmframe_equal_bgr_on_cv2_decode(layout, form):
     """One-frame crops, boxes partly outside the frame included, at every output layout."""
     from fastmot_b200 import _lib
-    from fastmot_b200.devmem import ptr, stream_ptr
+    from fastmot_b200.devmem import Frame, ptr, stream_ptr
     lib = _lib.require_device()
     W, H = SIZES[0]
     nv, bgr = _nv12_pair(SIZES[0], seed=5)
@@ -154,54 +155,61 @@ def test_crops_nv12_equal_bgr_on_cv2_decode(layout, form):
     shape = {0: (n, 3, oh, ow), 1: (n, oh, ow, 8), 2: (n, oh + 8, ow + 8, 4)}[layout]
     dt = torch.float32 if layout == 0 else torch.float16
     want, got = (torch.zeros(shape, dtype=dt, device="cuda") for _ in range(2))
-    bgr_dev = torch.as_tensor(bgr).cuda()
-    _lib.check(lib.fm_roi_resize_norm(ptr(bgr_dev), W, H, ptr(tl_dev), None, n, ow, oh, layout, ptr(want),
-                                      stream_ptr()), "fm_roi_resize_norm")
+    bgr_dev = Frame.bgr(torch.as_tensor(bgr).cuda())
+    _lib.check(lib.fm_roi_resize_norm(C.byref(bgr_dev.fm()), ptr(tl_dev), None, n, ow, oh, layout, ptr(want),
+                                      stream_ptr()), "fm_roi_resize_norm BGR")
     f = _frame(nv, form)
-    _lib.check(lib.fm_roi_resize_norm_nv12(*f.nv12_args(), W, H, ptr(tl_dev), None, n, ow, oh, layout, ptr(got),
-                                           stream_ptr()), "fm_roi_resize_norm_nv12")
+    assert f.size == (W, H)
+    _lib.check(lib.fm_roi_resize_norm(C.byref(f.fm()), ptr(tl_dev), None, n, ow, oh, layout, ptr(got), stream_ptr()),
+               "fm_roi_resize_norm NV12")
     assert _bits_equal(got, want)
 
 
 @pytest.mark.parametrize("form", FORMS)
-def test_gray_half_and_gray_resize_nv12(form):
+def test_gray_half_and_gray_resize_nv12_fmframe(form):
     """gray_half at 1080p (2x2 block = one chroma sample) and gray_resize at optical-flow scale 0.6 x 0.45."""
     from fastmot_b200 import _lib
-    from fastmot_b200.devmem import ptr, stream_ptr
+    from fastmot_b200.devmem import Frame, ptr, stream_ptr
     lib = _lib.require_device()
     W, H = SIZES[0]
     nv, bgr = _nv12_pair(SIZES[0], seed=9)
-    bgr_dev = torch.as_tensor(bgr).cuda()
+    bgr_dev = Frame.bgr(torch.as_tensor(bgr).cuda())
+    bgr_fm = C.byref(bgr_dev.fm())
     f = _frame(nv, form)
+    assert f.size == (W, H)
+    nv_fm = C.byref(f.fm())
     for sw, sh in ((W // 2, H // 2), (round(0.6 * W), round(0.45 * H))):
         g_want, g_got = (torch.zeros(H, W, dtype=torch.uint8, device="cuda") for _ in range(2))
         s_want, s_got = (torch.zeros(sh, sw, dtype=torch.uint8, device="cuda") for _ in range(2))
         if 2 * sw == W:
-            _lib.check(lib.fm_gray_half(ptr(bgr_dev), W, H, ptr(g_want), ptr(s_want), stream_ptr()), "gray_half")
-            _lib.check(lib.fm_gray_half_nv12(*f.nv12_args(), W, H, ptr(g_got), ptr(s_got), stream_ptr()),
-                       "gray_half_nv12")
+            _lib.check(lib.fm_gray_half(bgr_fm, ptr(g_want), ptr(s_want), stream_ptr()), "gray_half BGR")
+            _lib.check(lib.fm_gray_half(nv_fm, ptr(g_got), ptr(s_got), stream_ptr()), "gray_half NV12")
         else:
-            _lib.check(lib.fm_gray_resize(ptr(bgr_dev), W, H, ptr(g_want), ptr(s_want), sw, sh, stream_ptr()),
-                       "gray_resize")
-            _lib.check(lib.fm_gray_resize_nv12(*f.nv12_args(), W, H, ptr(g_got), ptr(s_got), sw, sh, stream_ptr()),
-                       "gray_resize_nv12")
+            _lib.check(lib.fm_gray_resize(bgr_fm, ptr(g_want), ptr(s_want), sw, sh, stream_ptr()), "gray_resize BGR")
+            _lib.check(lib.fm_gray_resize(nv_fm, ptr(g_got), ptr(s_got), sw, sh, stream_ptr()), "gray_resize NV12")
         assert _bits_equal(g_got, g_want), (sw, sh)
         assert _bits_equal(s_got, s_want), (sw, sh)
         want = cv2.cvtColor(bgr, cv2.COLOR_BGR2GRAY)
         assert np.array_equal(g_want.cpu().numpy(), want)
 
 
-def test_nv12_entry_points_reject_odd_sizes_and_short_pitches():
+def test_frame_descriptor_rejects_bad_nv12_and_null_bgr():
+    """NV12 frames with an odd size, a short pitch or no UV plane, and a BGR frame without pixels, are rejected."""
     from fastmot_b200 import _lib
     from fastmot_b200.devmem import ptr, stream_ptr
     lib = _lib.require_device()
     buf = torch.zeros(4096, dtype=torch.uint8, device="cuda")
     out = torch.zeros(4096, dtype=torch.uint8, device="cuda")
-    p = ptr(buf)
-    assert lib.fm_gray_half_nv12(p, p, 32, 32, 31, 16, ptr(out), ptr(out), stream_ptr()) != 0
-    assert lib.fm_gray_resize_nv12(p, p, 32, 32, 32, 15, ptr(out), ptr(out), 16, 8, stream_ptr()) != 0
-    assert lib.fm_gray_half_nv12(p, p, 30, 32, 32, 16, ptr(out), ptr(out), stream_ptr()) != 0
-    assert lib.fm_letterbox_preproc_nv12(p, None, 32, 32, 32, 16, 8, 8, 0, 0, 8, 8, 1, ptr(out), stream_ptr()) != 0
+    p = buf.data_ptr()
+
+    def fm(y, uv, w, h, pitch, uv_pitch, fmt=_lib.FM_PIX_NV12):
+        return C.byref(_lib.FmFrame(y, uv, w, h, pitch, uv_pitch, fmt))
+    assert lib.fm_gray_half(fm(p, p, 31, 16, 32, 32), ptr(out), ptr(out), stream_ptr()) != 0
+    assert lib.fm_gray_resize(fm(p, p, 32, 15, 32, 32), ptr(out), ptr(out), 16, 8, stream_ptr()) != 0
+    assert lib.fm_gray_half(fm(p, p, 32, 16, 30, 32), ptr(out), ptr(out), stream_ptr()) != 0
+    assert lib.fm_letterbox_preproc(fm(p, None, 32, 16, 32, 32), 8, 8, 0, 0, 8, 8, 1, ptr(out), stream_ptr()) != 0
+    assert lib.fm_letterbox_preproc(fm(None, None, 32, 16, 0, 0, _lib.FM_PIX_BGR), 8, 8, 0, 0, 8, 8, 1, ptr(out),
+                                    stream_ptr()) != 0
 
 
 # ------------------------------------------------------------------------------------------------ end to end

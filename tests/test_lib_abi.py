@@ -75,7 +75,7 @@ def test_ctypes_struct_layouts_match_the_header(tmp_path):
         pytest.skip("no C compiler")
     structs = [getattr(_lib, n) for n in dir(_lib)
                if n.startswith("Fm") and isinstance(getattr(_lib, n), type) and issubclass(getattr(_lib, n), ctypes.Structure)]
-    assert len(structs) >= 9
+    assert len(structs) >= 9 and _lib.FmFrame in structs and _lib.FmFrameGeom in structs
     lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "fastmot_b200.h"', 'int main(void) {']
     for st in structs:
         lines.append(f'  printf("{st.__name__} %zu\\n", sizeof({st.__name__}));')
