@@ -158,138 +158,12 @@ __global__ void find_occluded_kernel(const double* __restrict__ tlbr, int n, dou
     out[i] = occ;
 }
 
-// ----------------------------------------------------------------------------------------------------------
-// Rectangular LSA, one warp.  Replays SciPy's shortest-augmenting-path solver: `remaining` is filled in
-// reverse and compacted by swap-with-last; among equal minima the LAST unassigned column in scan order wins,
-// otherwise the FIRST minimum; doubles are combined in SciPy's order ((minVal + c) - u) - v.
-// ----------------------------------------------------------------------------------------------------------
-struct LsaBufs {
-    double *u, *v, *spc;
-    int *path, *col4row, *row4col, *remaining;
-    unsigned char *SR, *SC;
-};
-
-__device__ __forceinline__ LsaBufs lsa_carve(unsigned char* base, int nr, int nc) {
-    LsaBufs b;
-    size_t off = 0;
-    b.u = (double*)(base + off); off += sizeof(double) * nr;
-    b.v = (double*)(base + off); off += sizeof(double) * nc;
-    b.spc = (double*)(base + off); off += sizeof(double) * nc;
-    b.path = (int*)(base + off); off += sizeof(int) * nc;
-    b.col4row = (int*)(base + off); off += sizeof(int) * nr;
-    b.row4col = (int*)(base + off); off += sizeof(int) * nc;
-    b.remaining = (int*)(base + off); off += sizeof(int) * nc;
-    b.SR = base + off; off += nr;
-    b.SC = base + off;
-    return b;
-}
-
-__host__ __device__ inline size_t lsa_bytes(int nr, int nc) {
+// Solver state of lsa_block_kernel (the layout carve() in assoc_lsa_block.cu cuts), 16-byte rounded: it decides
+// between shared memory and the caller's workspace.
+inline size_t lsa_bytes(int nr, int nc) {
     size_t s = sizeof(double) * ((size_t)nr + 2 * (size_t)nc) + sizeof(int) * ((size_t)nr + 3 * (size_t)nc) +
                (size_t)nr + (size_t)nc;
     return (s + 15) & ~(size_t)15;
-}
-
-__global__ void __launch_bounds__(32) lsa_kernel(const double* __restrict__ cost, int nr0, int nc0,
-                                                  int* __restrict__ out_col4row, int* __restrict__ status,
-                                                  unsigned char* gws, int use_smem) {
-    extern __shared__ __align__(16) unsigned char s_ws[];
-    const int lane = threadIdx.x;
-    const bool transpose = nc0 < nr0;
-    const int nr = transpose ? nc0 : nr0;
-    const int nc = transpose ? nr0 : nc0;
-    LsaBufs B = lsa_carve(use_smem ? s_ws : gws, nr, nc);
-#define COST(i, j) (transpose ? cost[(size_t)(j) * nc0 + (i)] : cost[(size_t)(i) * nc0 + (j)])
-    for (int k = lane; k < nr; k += 32) { B.u[k] = 0.0; B.col4row[k] = -1; }
-    for (int k = lane; k < nc; k += 32) { B.v[k] = 0.0; B.row4col[k] = -1; B.path[k] = -1; }
-    if (lane == 0) status[0] = 0;
-    __syncwarp();
-    bool infeasible = false;
-    for (int curRow = 0; curRow < nr && !infeasible; ++curRow) {
-        for (int k = lane; k < nc; k += 32) { B.remaining[k] = nc - k - 1; B.SC[k] = 0; B.spc[k] = INFINITY; }
-        for (int k = lane; k < nr; k += 32) B.SR[k] = 0;
-        __syncwarp();
-        int num_remaining = nc;
-        double minVal = 0.0;
-        int i = curRow, sink = -1;
-        while (sink == -1) {
-            if (lane == 0) B.SR[i] = 1;
-            const double ui = B.u[i];
-            double l_min = INFINITY;
-            int l_first = 0x7fffffff, l_lastU = -1;
-            for (int it = lane; it < num_remaining; it += 32) {
-                int j = B.remaining[it];
-                double r = __dsub_rn(__dsub_rn(__dadd_rn(minVal, COST(i, j)), ui), B.v[j]);
-                double s = B.spc[j];
-                if (r < s) { B.path[j] = i; B.spc[j] = r; s = r; }
-                bool un = B.row4col[j] == -1;
-                if (s < l_min) { l_min = s; l_first = it; l_lastU = un ? it : -1; }
-                else if (s == l_min) { if (l_first == 0x7fffffff) l_first = it; if (un) l_lastU = it; }
-            }
-            double m = l_min;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) m = fmin(m, __shfl_xor_sync(0xffffffffu, m, o));
-            int c_first = (l_min == m) ? l_first : 0x7fffffff;
-            int c_lastU = (l_min == m) ? l_lastU : -1;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                c_first = min(c_first, __shfl_xor_sync(0xffffffffu, c_first, o));
-                c_lastU = max(c_lastU, __shfl_xor_sync(0xffffffffu, c_lastU, o));
-            }
-            if (m == INFINITY) { infeasible = true; break; }
-            minVal = m;
-            int index = (c_lastU >= 0) ? c_lastU : c_first;
-            int j = B.remaining[index];
-            int r4c = B.row4col[j];
-            if (r4c == -1) sink = j; else i = r4c;
-            __syncwarp();
-            if (lane == 0) {
-                B.SC[j] = 1;
-                B.remaining[index] = B.remaining[num_remaining - 1];
-            }
-            --num_remaining;
-            __syncwarp();
-        }
-        if (infeasible) break;
-        // dual update
-        if (lane == 0) B.u[curRow] = __dadd_rn(B.u[curRow], minVal);
-        for (int k = lane; k < nr; k += 32)
-            if (B.SR[k] && k != curRow) B.u[k] = __dadd_rn(B.u[k], __dsub_rn(minVal, B.spc[B.col4row[k]]));
-        for (int k = lane; k < nc; k += 32)
-            if (B.SC[k]) B.v[k] = __dsub_rn(B.v[k], __dsub_rn(minVal, B.spc[k]));
-        __syncwarp();
-        if (lane == 0) {
-            int j = sink;
-            while (true) {
-                int ii = B.path[j];
-                B.row4col[j] = ii;
-                int tmp = B.col4row[ii];
-                B.col4row[ii] = j;
-                j = tmp;
-                if (ii == curRow) break;
-            }
-        }
-        __syncwarp();
-    }
-    if (infeasible) {
-        if (lane == 0) status[0] = 1;
-        for (int k = lane; k < nr0; k += 32) out_col4row[k] = -1;
-        return;
-    }
-    if (!transpose) {
-        for (int k = lane; k < nr0; k += 32) {
-            int c = B.col4row[k];
-            if (c >= 0 && cost[(size_t)k * nc0 + c] >= FM_INF_COST) c = -2 - c;
-            out_col4row[k] = c;
-        }
-    } else {
-        for (int k = lane; k < nr0; k += 32) {  // original rows are the columns of the transposed problem
-            int c = B.row4col[k];
-            if (c >= 0 && cost[(size_t)k * nc0 + c] >= FM_INF_COST) c = -2 - c;
-            out_col4row[k] = c;
-        }
-    }
-#undef COST
 }
 
 // ----------------------------------------------------------------------------------------------------------
@@ -454,12 +328,8 @@ extern "C" int fm_lsa(const double* cost, int nr, int nc, int* col4row, int* sta
     size_t bytes = lsa_bytes(a, b);
     int use_smem = bytes <= 46 * 1024;
     FM_REQUIRE(use_smem || workspace, "fm_lsa: workspace required for this size");
-    if (b > 48 || getenv("FM_LSA_V1") == nullptr)   // <= 256 columns: one warp, state in registers (assoc_lsa_block.cu)
-        fm_launch_lsa_block(cost, nr, nc, col4row, status, (unsigned char*)workspace, use_smem, bytes,
-                            (cudaStream_t)stream);
-    else
-        lsa_kernel<<<1, 32, use_smem ? bytes : 0, (cudaStream_t)stream>>>(cost, nr, nc, col4row, status,
-                                                                          (unsigned char*)workspace, use_smem);
+    fm_launch_lsa_block(cost, nr, nc, col4row, status, (unsigned char*)workspace, use_smem, bytes,
+                        (cudaStream_t)stream);
     FM_CHECK_LAUNCH("fm_lsa");
     return FM_OK;
 }

@@ -1,9 +1,9 @@
-// Rectangular LSA with a whole CTA (one thread per remaining column): same replay of SciPy's
-// shortest-augmenting-path solver as lsa_kernel in assoc.cu (scan order of `remaining`, swap-with-last compaction,
-// "last unassigned among equal minima, else first minimum", fp64 operation order), but the per-step scan, the dual
-// update and the resets run across up to 1024 threads instead of one warp.  Bit-exact by construction: every
-// floating-point expression is evaluated by exactly one thread in SciPy's order; only the (associative) min / index
-// selection is parallel.
+// Rectangular LSA with a whole CTA (one thread per remaining column): a replay of SciPy's shortest-augmenting-path
+// solver (`remaining` is filled in reverse and compacted by swap-with-last; among equal minima the LAST unassigned
+// column in scan order wins, otherwise the FIRST minimum; doubles are combined in SciPy's order
+// ((minVal + c) - u) - v), with the per-step scan, the dual update and the resets spread over up to 1024 threads.
+// Bit-exact by construction: every floating-point expression is evaluated by exactly one thread in SciPy's order;
+// only the (associative) min / index selection is parallel.
 #include "common.cuh"
 #include "../../include/fastmot_b200.h"
 #include "assoc_lsa.cuh"
@@ -291,18 +291,14 @@ __global__ void __launch_bounds__(32) lsa_warp_kernel(const double* __restrict__
 int fm_launch_lsa_block(const double* cost, int nr, int nc, int* col4row, int* status, unsigned char* ws, int use_smem,
                         size_t smem_bytes, cudaStream_t s) {
     const int big = nr > nc ? nr : nc;
-    static int v1 = -1;            // FM_LSA_V1=1: previous CTA-wide kernel (A/B timing)
-    if (v1 < 0) { const char* e = getenv("FM_LSA_V1"); v1 = (e && e[0] == '1') ? 1 : 0; }
-    static int v2 = -1;            // FM_LSA_V2=1: block kernel v2 also below 257 columns (A/B timing)
-    if (v2 < 0) { const char* e = getenv("FM_LSA_V2"); v2 = (e && e[0] == '1') ? 1 : 0; }
-    if (big <= 256 && !v1 && !v2) {
+    if (big <= 256) {
         if (big <= 32) lsa_warp_kernel<1><<<1, 32, 0, s>>>(cost, nr, nc, col4row, status);
         else if (big <= 64) lsa_warp_kernel<2><<<1, 32, 0, s>>>(cost, nr, nc, col4row, status);
         else if (big <= 128) lsa_warp_kernel<4><<<1, 32, 0, s>>>(cost, nr, nc, col4row, status);
         else lsa_warp_kernel<8><<<1, 32, 0, s>>>(cost, nr, nc, col4row, status);
         return 0;
     }
-    if (big <= 1024 && !v1) {
+    if (big <= 1024) {
         int t2 = 64;
         while (t2 < big) t2 <<= 1;
         lsa_v2_kernel<<<1, t2, 0, s>>>(cost, nr, nc, col4row, status);

@@ -46,11 +46,8 @@ static inline int fm_cdiv(long long a, long long b) { return (int)((a + b - 1) /
 //   * fm_pdl_trigger() first thing in the CTA (the dependent grid may be scheduled once every CTA of this grid runs),
 //   * fm_pdl_wait() unconditionally, before the first access to memory another kernel produces or consumes; it
 //     returns only when the preceding grid has completed and flushed, so ordering stays transitive along the stream.
-// FM_PDL=0 in the environment launches everything fully serialised (A/B timing, debugging).
 __device__ __forceinline__ void fm_pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void fm_pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
-extern "C" int fm_pdl_enabled();
 
 template <typename... KArgs, typename... Args>
 static inline cudaError_t fm_launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s,
@@ -64,7 +61,7 @@ static inline cudaError_t fm_launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = fm_pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 

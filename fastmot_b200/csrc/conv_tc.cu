@@ -23,7 +23,6 @@
 #include "tc_common.cuh"
 #include "../../include/fastmot_b200.h"
 #include "conv_act.cuh"
-#include <stdlib.h>
 
 namespace {
 
@@ -460,13 +459,8 @@ int launch_tc(const FmConvDesc* d, const void* in, const void* wgt, const float*
     int sps = nk;
     // split-K when the output tiling alone cannot fill the SMs (batch-1 deep layers)
     const int tiles = grid.x * grid.y;
-    static int split_max_tiles = -1;     // FM_CONV_SPLIT_MAXTILES overrides the largest tile count that still splits K
-    if (split_max_tiles < 0) {
-        const char* e = getenv("FM_CONV_SPLIT_MAXTILES");
-        split_max_tiles = e ? atoi(e) : FM_NUM_SMS / 2;
-    }
     float* ws = (float*)d->ws;
-    if (ws && tiles <= split_max_tiles && nk >= 8) {
+    if (ws && tiles <= FM_NUM_SMS / 2 && nk >= 8) {
         // as many K splits as still fit in ONE wave of resident CTAs: one CTA more than the SMs hold runs after the
         // others and doubles the layer time
         constexpr int per_sm = (227 * 1024) / (smem_split + 1024) > 0 ? (227 * 1024) / (smem_split + 1024) : 1;
@@ -519,8 +513,6 @@ extern "C" int fm_conv2d_tc(const FmConvDesc* d, const void* in, const void* wgt
     const int m_tiles_all = (d->n * d->ho * d->wo + TC_BM - 1) / TC_BM;
     // ring depth follows the K extent: short reductions (OSNet 1x1) want many co-resident CTAs, long ones (3x3 on
     // wide layers) want many slices of copies in flight
-    static int force_bn = -1;      // FM_CONV_BN=32|64|128 overrides the tile width (experiments only)
-    if (force_bn < 0) { const char* e = getenv("FM_CONV_BN"); force_bn = e ? atoi(e) : 0; }
     int bn = d->cout <= 32 ? 32 : d->cout <= 64 ? 64 : 128;
     if (bn == 128) {
         // between half a wave and two waves of 128-wide tiles, 64-wide tiles fill the SMs better (e.g.
@@ -528,31 +520,28 @@ extern "C" int fm_conv2d_tc(const FmConvDesc* d, const void* in, const void* wgt
         const int tiles128 = m_tiles_all * ((d->cout + 127) / 128);
         if (tiles128 > FM_NUM_SMS / 2 && tiles128 < 2 * FM_NUM_SMS) bn = 64;
     }
-    if (force_bn) bn = force_bn;
     // Ring depth: deep rings hide the gather latency of a long K loop, but they cost residency (6 x 32 KB = one CTA
     // per SM).  What decides is how the tile count sits against one wave of resident CTAs:
     //   * the layer fits in one wave at the deep setting          -> deep ring (and split-K fills the idle SMs),
     //   * it fits in one wave only with a shallower ring          -> that ring (a second, mostly empty wave doubles
     //                                                                the layer time),
     //   * many waves either way (OSNet stem, first YOLO layers)   -> shallow ring, residency hides the latency.
-    static int rules = -1;          // FM_CONV_RULES=0 restores the K-only rule (A/B timing)
-    if (rules < 0) { const char* e = getenv("FM_CONV_RULES"); rules = (e && e[0] == '0') ? 0 : 1; }
     const int tiles = m_tiles_all * ((d->cout + bn - 1) / bn);
     if (bn == 32) {
         if (nk == 1) launch_tc<32, 1>(d, in, wgt, bias, residual, out, s);
-        else if (nk <= 2 || (rules && tiles > 5 * FM_NUM_SMS)) launch_tc<32, 2>(d, in, wgt, bias, residual, out, s);
+        else if (nk <= 2 || tiles > 5 * FM_NUM_SMS) launch_tc<32, 2>(d, in, wgt, bias, residual, out, s);
         else launch_tc<32, 4>(d, in, wgt, bias, residual, out, s);
     } else if (bn == 64) {
         // 64-wide: 4 stages = 96 KB (2 CTAs / SM), 2 stages = 48 KB (4 / SM)
         if (nk == 1) launch_tc<64, 1>(d, in, wgt, bias, residual, out, s);
-        else if (nk <= 2 || (rules ? tiles > 2 * FM_NUM_SMS : m_tiles_all >= 8 * FM_NUM_SMS))
+        else if (nk <= 2 || tiles > 2 * FM_NUM_SMS)
             launch_tc<64, 2>(d, in, wgt, bias, residual, out, s);   // e.g. the OSNet 7x7 stem
         else launch_tc<64, 4>(d, in, wgt, bias, residual, out, s);
     } else {
         // 128-wide: 6 stages = 192 KB (1 CTA / SM), 3 stages = 96 KB (2 / SM), 2 stages = 64 KB (3 / SM)
         if (nk == 1) launch_tc<128, 1>(d, in, wgt, bias, residual, out, s);
-        else if (nk <= 2 || (rules && tiles > 2 * FM_NUM_SMS)) launch_tc<128, 2>(d, in, wgt, bias, residual, out, s);
-        else if (nk < 6 || (rules && tiles > FM_NUM_SMS)) launch_tc<128, 3>(d, in, wgt, bias, residual, out, s);
+        else if (nk <= 2 || tiles > 2 * FM_NUM_SMS) launch_tc<128, 2>(d, in, wgt, bias, residual, out, s);
+        else if (nk < 6 || tiles > FM_NUM_SMS) launch_tc<128, 3>(d, in, wgt, bias, residual, out, s);
         else launch_tc<128, 6>(d, in, wgt, bias, residual, out, s);
     }
     FM_CHECK_LAUNCH("fm_conv2d_tc");

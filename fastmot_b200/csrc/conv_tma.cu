@@ -401,12 +401,6 @@ int max_clusters(int s) {
     return n;
 }
 
-int verbose() {
-    static int v = -1;                   // FM_CONV_TMA_VERBOSE=1: one line per planned launch on stderr
-    if (v < 0) { const char* e = getenv("FM_CONV_TMA_VERBOSE"); v = (e && e[0] == '1') ? 1 : 0; }
-    return v;
-}
-
 int split_limit() {
     static int v = -1;                   // FM_CONV_TMA_SPLIT=<n>: upper bound of the cluster size (1 = never split K)
     if (v < 0) { const char* e = getenv("FM_CONV_TMA_SPLIT"); v = e ? atoi(e) : 8; if (v < 1) v = 1; if (v > 8) v = 8; }
@@ -425,7 +419,7 @@ int pick_split(int tiles, int nk) {
 }
 
 template <int BN>
-int launch_tma(const FmConvDesc* d, const Plan& p, int S, bool deep, const void* in, const void* wgt, const float* bias,
+int launch_tma(const FmConvDesc* d, const Plan& p, int S, const void* in, const void* wgt, const float* bias,
                const void* residual, void* out, cudaStream_t st) {
     const int kc = d->cin / 64, taps = d->kh * d->kw, nk = taps * kc;
     const int ncol = fm_cdiv(d->cout, BN);
@@ -433,7 +427,7 @@ int launch_tma(const FmConvDesc* d, const Plan& p, int S, bool deep, const void*
     int sps = fm_cdiv(nk, S);
     S = fm_cdiv(nk, sps);
     // ring depth: as deep as one CTA per SM allows next to the slots of a cluster
-    const int ns = !deep ? (BN == 128 ? 3 : 4) : S > 1 ? (BN == 128 ? 4 : 7) : (BN == 128 ? 6 : 8);
+    const int ns = S > 1 ? (BN == 128 ? 4 : 7) : (BN == 128 ? 6 : 8);
     const int smem_total = smem_bytes<BN>(ns, S > 1);
     ConvTmaArgs a;
     a.W = p.W; a.H = p.H; a.TW = p.TW; a.TH = p.TH; a.tiles_w = p.tiles_w;
@@ -463,44 +457,20 @@ int launch_tma(const FmConvDesc* d, const Plan& p, int S, bool deep, const void*
     const uint64_t ktot = (uint64_t)taps * d->cin;
     rc = fm_make_tmap_f16_3d(&map_b, wgt, ktot, (uint64_t)d->cout, 1, ktot, ktot * d->cout, 64, BN, 1);
     if (rc) return rc;
-    if (verbose()) {
-        static bool once = false;
-        if (!once) {
-            once = true;
-            int smpm = 0, regs = 0;
-            cudaDeviceGetAttribute(&smpm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, 0);
-            cudaDeviceGetAttribute(&regs, cudaDevAttrMaxRegistersPerMultiprocessor, 0);
-            fprintf(stderr, "device: smem/SM %d, regs/SM %d; blocks/SM of conv_tma<%d> by dynamic smem:", smpm, regs, BN);
-            for (int kb = 32; kb <= 112; kb += 16) {
-                int bps = -1;
-                cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, conv_tma_kernel<BN>, kThreads, kb * 1024);
-                fprintf(stderr, " %dK:%d", kb, bps);
-            }
-            fprintf(stderr, "\n");
-        }
-    }
-    if (verbose())
-        fprintf(stderr, "conv_tma<%d> ring %d: %dx%d k%d s%d cin %d cout %d: rect %dx%d tiles %d x %d, nk %d, cluster %d (%d slices)\n",
-                BN, ns, p.W, p.H, d->kh, d->stride, d->cin, d->cout, p.TW, p.TH, p.tiles, ncol, nk, S, sps);
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(p.tiles, ncol, S);
     cfg.blockDim = dim3(kThreads);
     cfg.dynamicSmemBytes = smem_total;
     cfg.stream = st;
     cudaLaunchAttribute attrs[2];
-    int na = 0;
-    if (fm_pdl_enabled()) {
-        attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attrs[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
+    attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attrs[0].val.programmaticStreamSerializationAllowed = 1;
     if (S > 1) {
-        attrs[na].id = cudaLaunchAttributeClusterDimension;
-        attrs[na].val.clusterDim.x = 1; attrs[na].val.clusterDim.y = 1; attrs[na].val.clusterDim.z = S;
-        ++na;
+        attrs[1].id = cudaLaunchAttributeClusterDimension;
+        attrs[1].val.clusterDim.x = 1; attrs[1].val.clusterDim.y = 1; attrs[1].val.clusterDim.z = S;
     }
     cfg.attrs = attrs;
-    cfg.numAttrs = na;
+    cfg.numAttrs = S > 1 ? 2 : 1;
     cudaError_t e = cudaLaunchKernelEx(&cfg, conv_tma_kernel<BN>, map_a, map_b, a, ns);
     if (e != cudaSuccess) { fm_set_last_error(cudaGetErrorString(e)); return FM_ERR_CUDA; }
     return FM_OK;
@@ -544,21 +514,16 @@ extern "C" int fm_conv2d_tma(const FmConvDesc* d, const void* in, const void* wg
     const Plan p = plan_tiles(d);
     const int nk = d->kh * d->kw * (d->cin / 64);
     // 64-wide filter tiles when 128-wide ones (with the deepest K split the layer allows) would leave half the GPU idle
-    static int force_bn = -1;            // FM_CONV_TMA_BN=64|128 (experiments)
-    if (force_bn < 0) { const char* e = getenv("FM_CONV_TMA_BN"); force_bn = e ? atoi(e) : 0; }
-    static int deep = -1;                // FM_CONV_TMA_DEEP=0: never use the deep-ring instantiations
-    if (deep < 0) { const char* e = getenv("FM_CONV_TMA_DEEP"); deep = (e && e[0] == '0') ? 0 : 1; }
     int bn = d->cout >= 128 ? 128 : 64;
     if (bn == 128) {
         const int smax = nk / 2 < 8 ? (nk / 2 < 1 ? 1 : nk / 2) : 8;
         if ((long long)p.tiles * fm_cdiv(d->cout, 128) * smax <= FM_NUM_SMS / 2) bn = 64;
     }
-    if (force_bn == 64 || force_bn == 128) bn = force_bn;
     const int tiles = p.tiles * fm_cdiv(d->cout, bn);
     int rc;
     const int S = bn == 128 ? pick_split<128>(tiles, nk) : pick_split<64>(tiles, nk);
-    rc = bn == 128 ? launch_tma<128>(d, p, S, deep != 0, in, wgt, bias, residual, out, st)
-                   : launch_tma<64>(d, p, S, deep != 0, in, wgt, bias, residual, out, st);
+    rc = bn == 128 ? launch_tma<128>(d, p, S, in, wgt, bias, residual, out, st)
+                   : launch_tma<64>(d, p, S, in, wgt, bias, residual, out, st);
     if (rc) return rc;
     FM_CHECK_LAUNCH("fm_conv2d_tma");
     return FM_OK;

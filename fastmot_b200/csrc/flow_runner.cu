@@ -7,8 +7,6 @@
 #include "../../include/fastmot_b200.h"
 #include <new>
 
-#include <stdlib.h>
-
 namespace {
 struct FlowRunner {
     FmFlowPlan p;
@@ -19,15 +17,6 @@ struct FlowRunner {
     int pyr_state[2] = {0, 0};
     int pyr_nodes = 0;
 };
-
-bool pyr_graph_enabled() {
-    static int on = -1;
-    if (on < 0) {
-        const char* e = getenv("FM_PYR_GRAPH");
-        on = (e && e[0] == '0') ? 0 : 1;
-    }
-    return on != 0;
-}
 
 // Records pyr_level / scharr of buffer k into a graph by stream capture on two private streams.  Any failure leaves
 // the runner on plain launches (state -1); nothing here touches the caller's streams.
@@ -129,13 +118,11 @@ int preprocess(FlowRunner* r, const FmFrame* f, int k, void* stream) {
         FM_TRY(fm_gray_half(f, p.gray[k], small, stream));
     else
         FM_TRY(fm_gray_resize(f, p.gray[k], small, py.w[0], py.h[0], stream));
-    if (pyr_graph_enabled()) {
-        if (r->pyr_state[k] == 0) build_pyr_graph(r, k);
-        if (r->pyr_state[k] == 1) {
-            FM_CUDA_TRY(cudaGraphLaunch(r->pyr_graph[k], (cudaStream_t)stream), "fm_flow_predict: pyramid graph");
-            fm_count_launches(r->pyr_nodes);
-            return FM_OK;
-        }
+    if (r->pyr_state[k] == 0) build_pyr_graph(r, k);
+    if (r->pyr_state[k] == 1) {
+        FM_CUDA_TRY(cudaGraphLaunch(r->pyr_graph[k], (cudaStream_t)stream), "fm_flow_predict: pyramid graph");
+        fm_count_launches(r->pyr_nodes);
+        return FM_OK;
     }
     for (int i = 0; i < py.n_levels; ++i) {
         if (i + 1 < py.n_levels)

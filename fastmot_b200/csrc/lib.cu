@@ -1,4 +1,3 @@
-#include <stdlib.h>
 // Library-level entry points: error string, version, device probe.
 #include "common.cuh"
 #include "../../include/fastmot_b200.h"
@@ -58,13 +57,3 @@ extern "C" int fm_host_is_pinned(const void* p) {
 static long long g_launches = 0;
 extern "C" void fm_count_launches(int n) { __atomic_fetch_add(&g_launches, (long long)n, __ATOMIC_RELAXED); }
 extern "C" long long fm_launch_count(void) { return __atomic_load_n(&g_launches, __ATOMIC_RELAXED); }
-
-// Programmatic dependent launch switch (common.cuh fm_launch_pdl); FM_PDL=0 disables it.
-extern "C" int fm_pdl_enabled() {
-    static int on = -1;
-    if (on < 0) {
-        const char* e = getenv("FM_PDL");
-        on = (e && e[0] == '0') ? 0 : 1;
-    }
-    return on;
-}

@@ -1,7 +1,6 @@
 // 16-byte vectorised versions of the bandwidth-bound NHWC fp16 layers (8 channels per thread).  Each `fm_vec_*`
 // returns 1 if it handled the call (all channel counts / strides / offsets multiples of 8), 0 otherwise — the
 // scalar kernels in nn.cu remain the general path.
-#include <cstdlib>
 #include "common.cuh"
 #include "../../include/fastmot_b200.h"
 
@@ -406,9 +405,7 @@ int fm_vec_dwconv3(const void* in, const void* w, const float* bias, void* out, 
     if (!al8(c)) return 0;
     if ((wd & 3) == 0) {
         const size_t tile_bytes = ((size_t)(DW_R + 2) * wd + 9) * c * sizeof(__half);
-        static int use_tile = -1;          // FM_DW_TILE=0 falls back to the untiled kernel (A/B timing only)
-        if (use_tile < 0) { const char* e = getenv("FM_DW_TILE"); use_tile = (e && e[0] == '0') ? 0 : 1; }
-        if (use_tile && tile_bytes <= 96 * 1024 && h >= DW_R) {
+        if (tile_bytes <= 96 * 1024 && h >= DW_R) {
             static size_t attr_bytes = 0;
             if (tile_bytes > attr_bytes) {
                 cudaFuncSetAttribute(dwconv3_tile, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(96 * 1024));

@@ -419,19 +419,14 @@ int launch_streams(const FmOsbStreams* d, cudaStream_t st) {
     cfg.dynamicSmemBytes = C::SMEM;
     cfg.stream = st;
     cudaLaunchAttribute attrs[2];
-    int na = 0;
-    if (fm_pdl_enabled()) {
-        attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-        attrs[na].val.programmaticStreamSerializationAllowed = 1;
-        ++na;
-    }
+    attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attrs[0].val.programmaticStreamSerializationAllowed = 1;
     if (CL > 1) {
-        attrs[na].id = cudaLaunchAttributeClusterDimension;
-        attrs[na].val.clusterDim.x = CL; attrs[na].val.clusterDim.y = 1; attrs[na].val.clusterDim.z = 1;
-        ++na;
+        attrs[1].id = cudaLaunchAttributeClusterDimension;
+        attrs[1].val.clusterDim.x = CL; attrs[1].val.clusterDim.y = 1; attrs[1].val.clusterDim.z = 1;
     }
     cfg.attrs = attrs;
-    cfg.numAttrs = na;
+    cfg.numAttrs = CL > 1 ? 2 : 1;
     cudaError_t e = cudaLaunchKernelEx(&cfg, osb_streams_kernel<W, MID, T, NS, CL>, map, a);
     if (e != cudaSuccess) { fm_set_last_error(cudaGetErrorString(e)); return FM_ERR_CUDA; }
     return FM_OK;
@@ -683,10 +678,7 @@ extern "C" int fm_osb_set_debug(void* dbg) {     // debugging aid, not part of t
 }
 
 extern "C" int fm_osb_streams_strips(int h, int w, int mid) {
-    if (w == 32 && mid == 64 && h == 64) {
-        const char* e = getenv("FM_OSB_CLUSTER");
-        if (!(e && e[0] == '0')) return 4;          // one 4-CTA cluster per crop
-    }
+    if (w == 32 && mid == 64 && h == 64) return 4;  // one 4-CTA cluster per crop
     if (w == 32 && mid == 64) return h == 16 ? 1 : (h % 8 == 0 && h > 16 ? h / 8 : 0);   // 16 rows = one strip, no halo
     if (w == 16 && mid == 96 && h == 32) return 2;  // two-CTA cluster per crop
     if (w == 8 && mid == 128) return h == 16 ? 1 : 0;
@@ -700,8 +692,8 @@ extern "C" int fm_osb_streams(const FmOsbStreams* d, void* stream) {
     if (d->n <= 0) return FM_OK;
     cudaStream_t st = (cudaStream_t)stream;
     int rc;
-    // stage 1 (32 x 64): a 4-CTA cluster per crop, or (FM_OSB_CLUSTER=0) strips with a recomputed 4-row halo
-    if (d->w == 32 && fm_osb_streams_strips(d->h, d->w, d->mid) == 4 && d->h == 64) rc = launch_streams<32, 64, 4, 3, 4>(d, st);
+    // stage 1 (w 32): a 4-CTA cluster per 64-row crop, other heights as strips (fm_osb_streams_strips)
+    if (d->w == 32 && d->h == 64) rc = launch_streams<32, 64, 4, 3, 4>(d, st);
     else if (d->w == 32) rc = launch_streams<32, 64, 4, 3, 1>(d, st);
     else if (d->w == 16) rc = launch_streams<16, 96, 2, 2, 2>(d, st);       // two 16-row strips per crop
     else rc = launch_streams<8, 128, 1, 2, 1>(d, st);

@@ -234,11 +234,10 @@ class YoloEngine(_Net):
                     refs.setdefault(s_, set()).add(i)
             elif l['type'] == 'shortcut':
                 refs.setdefault(l['from_abs'], set()).add(i)
-        fuse_sc = os.environ.get("FM_FUSE_SHORTCUT", "1") != "0"
         self.fused_shortcuts = set()
         for i, l in enumerate(L[:-1]):
             nx = L[i + 1]
-            if fuse_sc and l['type'] == 'convolutional' and nx['type'] == 'shortcut' and i not in home and \
+            if l['type'] == 'convolutional' and nx['type'] == 'shortcut' and i not in home and \
                     nx.get('activation', 'linear') == 'linear' and not refs.get(i) and nx['from_abs'] < i and \
                     self.shapes[nx['from_abs']] == self.shapes[i]:
                 self.fused_shortcuts.add(i + 1)
@@ -394,7 +393,7 @@ class OSNetEngine(_Net):
         super().__init__(use_tc, use_graph)
         # The ReID stack's stand-alone convs are thousands of tiles with 1-8 K slices each: the one-tile-per-CTA TMA
         # kernel pays its per-CTA set-up many times per SM there; it is the batch-1 detector layers it was written for.
-        self.use_tma = os.environ.get("FM_OSNET_TMA", "0") == "1"
+        self.use_tma = False
         if ops is not None and weights is None:
             raise ValueError("a custom op list needs its weights")
         self.ops = list(ops) if ops is not None else osnet.build_osnet(width, feature_dim)
@@ -408,8 +407,8 @@ class OSNetEngine(_Net):
         # fm_osb_streams + fm_osb_merge pair per OSBlock (csrc/osnet_fused.cu, csrc/osnet_stem.cu)
         self.fuse_osb = os.environ.get("FM_OSB_FUSED", "1") != "0" and use_tc
         first, second = self.ops[0], self.ops[1]
-        self.fuse_stem = (self.fuse_osb and os.environ.get("FM_OSB_STEM", "1") != "0" and (H, W) == (256, 128)
-                          and first[0] == 'conv' and first[2:8] == (3, 64, 7, 2, 3, 'relu') and second[0] == 'maxpool3s2'
+        self.fuse_stem = (self.fuse_osb and (H, W) == (256, 128) and first[0] == 'conv'
+                          and first[2:8] == (3, 64, 7, 2, 3, 'relu') and second[0] == 'maxpool3s2'
                           and second[1] == first[9])
         # network input: NHWC8 (layout 1 of fm_roi_resize_norm) or, for the fused stem, NHWC4 inside a zero border
         self.inp_layout = 2 if self.fuse_stem else 1

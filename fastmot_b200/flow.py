@@ -10,7 +10,6 @@ Kalman kernel reads directly.
 """
 import ctypes as C
 import logging
-import os
 
 import numpy as np
 import torch
@@ -189,8 +188,8 @@ class Flow:
     # ------------------------------------------------------------------ one-call runner (csrc/flow_runner.cu)
     def _plan(self):
         """Freezes every fixed buffer address and parameter of predict_device into an FmFlowPlan; the per-frame
-        enqueue is then a single C-ABI call (fm_flow_predict).  FM_FLOW_RUNNER=0, or an active stagetime pass (which
-        times the individual entry points), keeps the call-by-call sequence below."""
+        enqueue is then a single C-ABI call (fm_flow_predict).  An active stagetime pass (which times the individual
+        entry points) keeps the call-by-call sequence below."""
         pool = self.pool
         P = _lib.FmFlowPlan()
         W, H = self.size
@@ -254,7 +253,7 @@ class Flow:
             except Exception:
                 pass
 
-    USE_RUNNER = os.environ.get("FM_FLOW_RUNNER", "1") != "0"
+    USE_RUNNER = True       # False keeps the call-by-call sequence (tests compare the two)
 
     # ------------------------------------------------------------------ lazily fetched attributes
     def _fetch_bg(self):

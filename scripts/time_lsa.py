@@ -1,5 +1,5 @@
 """Times fm_lsa on tracker-like and random 200x200 cost matrices (CUDA events, median of 20).
-usage: python scripts/time_lsa.py   (FM_LSA_V1=1 selects the previous kernel)"""
+usage: python scripts/time_lsa.py"""
 import os
 import sys
 

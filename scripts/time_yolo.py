@@ -1,5 +1,5 @@
 """Times one detector conv-stack forward (CUDA events around the graph replay, L2 flushed between replays).
-usage: python scripts/time_yolo.py [model] [--eager]   (FM_CONV_TMA=0 / FM_FUSE_SHORTCUT=0 select the r01 path)"""
+usage: python scripts/time_yolo.py [model] [--eager]   (FM_CONV_TMA=0 puts every conv on the cp.async kernel)"""
 import os
 import sys
 
@@ -31,6 +31,6 @@ for _ in range(2 if eager else 20):
     ts.append(e0.elapsed_time(e1))
 ts.sort()
 med = ts[len(ts) // 2]
-print(f"{name} tma={os.environ.get('FM_CONV_TMA', '1')} fuse_shortcut={os.environ.get('FM_FUSE_SHORTCUT', '1')} "
+print(f"{name} tma={os.environ.get('FM_CONV_TMA', '1')} "
       f"convs tc={eng.n_tc} (tma {eng.n_tma}) simt={eng.n_simt} kernels={eng.kernels_per_replay()}: "
       f"median {med:.3f} ms  min {ts[0]:.3f}  max {ts[-1]:.3f}  {eng.flops / med / 1e9:.1f} TFLOP/s")

@@ -7,9 +7,6 @@ order differs from numpy's (8x8 products, 4x4 solves, dot products), bit-exact w
 occlusion, create, rounding, assignments).  Pools are filled with NaN-pattern sentinels so that a launch which reads
 or writes a slot it was not given is caught.  Each test prints its worst error / tolerance ratio under `pytest -s`.
 """
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -756,35 +753,6 @@ def test_lsa_workspace_path_vs_scipy(lib, shape):
     assert np.array_equal(c4r, want)
     assert n_dem == 3
     _report(f"lsa {shape} {'smem' if smem else 'workspace'}", bit_exact=True, demoted=n_dem)
-
-
-def _lsa_random_small():
-    """The random LSA shapes of test_gpu_assoc whose larger side is at most 48, against the oracle's SciPy replay."""
-    from gpu_util import run_lsa
-    from oracle import assoc
-    rng = np.random.default_rng(5)
-    for (nr, nc) in [(1, 1), (1, 9), (9, 1), (23, 23)]:
-        for mode in range(3):
-            if mode == 0:
-                C = rng.uniform(0, 1, (nr, nc))
-            elif mode == 1:
-                C = rng.integers(0, 3, (nr, nc)).astype(float)
-            else:
-                C = np.where(rng.uniform(size=(nr, nc)) < 0.6, INF, np.round(rng.uniform(0, 1, (nr, nc)), 2))
-            c4r, st = run_lsa(C)
-            assert st == 0
-            want, _ = _lsa_want(C, *assoc.lsa(C))
-            assert np.array_equal(c4r, want), (nr, nc, mode)
-
-
-def test_lsa_warp_kernel_env_switch():
-    """FM_LSA_V1=1 selects the one-warp kernel in assoc.cu for shapes whose larger side is at most 48; it must give
-    the same assignments as the oracle."""
-    code = "import sys; sys.path.insert(0, 'tests'); import test_gpu_assoc_sweep as t; t._lsa_random_small()"
-    env = dict(os.environ, FM_LSA_V1="1")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, "-c", code], cwd=root, env=env, capture_output=True, text=True, timeout=300)
-    assert r.returncode == 0, r.stderr[-2000:]
 
 
 def _run_cascade(lib, rng, n_det, sizes, n_unconf, n_hist, all_inf=False, feat_gated=0.35):

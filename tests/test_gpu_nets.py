@@ -154,7 +154,7 @@ TMA_CASES = [
 ]
 
 
-# conv_tma.cu epilogue with FM_ACT_AFTER_RESIDUAL; plans from fm_conv2d_tma / pick_split (FM_CONV_TMA_VERBOSE=1)
+# conv_tma.cu epilogue with FM_ACT_AFTER_RESIDUAL; plans from fm_conv2d_tma / pick_split
 RES_FIRST_TMA = [
     (4, 64, 32, 128, 128, 1, 1, 'leaky', 128, 0, 128, 0, True, True),  # 64-wide, 128 tiles, nk 2: S == 1, vector
     (1, 20, 20, 512, 256, 3, 1, 'leaky', 512, 0, 256, 0, True, True),  # 4 x 2 tiles, nk 72: S > 1, vector
