@@ -117,6 +117,7 @@ SIGNATURES = {
     "fm_roi_resize_norm": (c_i, [C.POINTER(FmFrame), c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p]),
     "fm_letterbox_preproc_geom": (c_i, [c_p, c_i, c_i, c_i, c_p, c_p]),
     "fm_roi_resize_norm_geom": (c_i, [c_p, c_p, c_p, c_i, c_i, c_i, c_i, c_p, c_p]),
+    "fm_frame_resize": (c_i, [C.POINTER(FmFrame), c_p, c_i, c_i, c_p]),
     "fm_yolo_decode_filter_geom": (c_i, [c_p, c_i, c_ll, c_i, c_i, c_i, c_i, c_i, C.POINTER(FmYoloHead), c_i, c_i,
                                           c_i, c_i, c_i, c_i, c_p, c_d, c_p, c_p, c_p, c_p, c_i, c_p]),
     "fm_diou_nms_filter_batch": (c_i, [c_i, c_p, c_p, c_i, c_p, c_i, c_d, c_d, c_d, c_p, c_i, c_p, c_p, c_p, c_p, c_p,

@@ -8,6 +8,7 @@
 #include "common.cuh"
 #include "../../include/fastmot_b200.h"
 #include "pixel_src.cuh"
+#include "cv_linear.cuh"
 
 namespace {
 
@@ -65,28 +66,18 @@ __global__ void __launch_bounds__(256) gray_kernel(Src src, int w, int h, unsign
 }
 
 // cv2.resize(src, (dw, dh)) INTER_LINEAR for u8 at a downscale (dw <= sw, dh <= sh): OpenCV's generic resize with
-// 11-bit coefficients (resize.cpp: scale = 1 / (dsize / ssize), coefficients rounded half to even, the vertical pass
-// of VResizeLinearVec_32s8u).  The source rows / columns are clamped at the far edge, where the weight is zero.
+// 11-bit coefficients (cv_linear.cuh, shared with fm_frame_resize).
 __global__ void __launch_bounds__(256) resize_linear_kernel(const unsigned char* __restrict__ src, int sw, int sh,
                                                              unsigned char* __restrict__ dst, int dw, int dh,
                                                              double scale_x, double scale_y) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y;
     if (x >= dw || y >= dh) return;
-    float fx = (float)((x + 0.5) * scale_x - 0.5), fy = (float)((y + 0.5) * scale_y - 0.5);
-    int sx = (int)floorf(fx), sy = (int)floorf(fy);
-    fx -= sx; fy -= sy;
-    if (sx < 0) { fx = 0; sx = 0; }
-    if (sx >= sw - 1) { fx = 0; sx = sw - 1; }
-    if (sy < 0) { fy = 0; sy = 0; }
-    if (sy >= sh - 1) { fy = 0; sy = sh - 1; }
-    const int a0 = (int)rintf((1.f - fx) * 2048.f), a1 = (int)rintf(fx * 2048.f);
-    const int b0 = (int)rintf((1.f - fy) * 2048.f), b1 = (int)rintf(fy * 2048.f);
-    const int sx1 = min(sx + 1, sw - 1), sy1 = min(sy + 1, sh - 1);
-    const unsigned char* r0 = src + (size_t)sy * sw;
-    const unsigned char* r1 = src + (size_t)sy1 * sw;
-    const int h0 = r0[sx] * a0 + r0[sx1] * a1, h1 = r1[sx] * a0 + r1[sx1] * a1;
-    dst[(size_t)y * dw + x] = (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2;
+    const FmLinearTap c = fm_linear_col(x, scale_x, sw), r = fm_linear_row(y, scale_y, sh);
+    const unsigned char* r0 = src + (size_t)r.i0 * sw;
+    const unsigned char* r1 = src + (size_t)r.i1 * sw;
+    const int h0 = r0[c.i0] * c.w0 + r0[c.i1] * c.w1, h1 = r1[c.i0] * c.w0 + r1[c.i1] * c.w1;
+    dst[(size_t)y * dw + x] = fm_linear_v(r, h0, h1);
 }
 
 __device__ __forceinline__ int reflect101(int p, int n) {

@@ -334,6 +334,47 @@ class UploadSlot:
         return up.upload_frame(f)
 
 
+def check_capture_size(capture_size, size, pixel_format):
+    """The (width, height) a tracker's frames arrive at: `size` (the tracking size) when capture_size is None, else
+    capture_size as a tuple of two positive ints (even for NV12).  Anything else raises ValueError."""
+    if capture_size is None:
+        return tuple(int(v) for v in size)
+    if not (isinstance(capture_size, (tuple, list)) and len(capture_size) == 2
+            and all(np.isscalar(v) and int(v) == v and v > 0 for v in capture_size)):
+        raise ValueError(f"capture_size must be (width, height) with positive integers, got {capture_size!r}")
+    w, h = (int(v) for v in capture_size)
+    if pixel_format == "NV12" and (w % 2 or h % 2):
+        raise ValueError(f"an NV12 capture size must be even, got {w}x{h}")
+    return w, h
+
+
+class FrameResizer:
+    """Device Frames of any size and format -> BGR Frames of one size (`size`, the tracking size): cv2.resize with the
+    default INTER_LINEAR of the frame (of its cv2.cvtColor decode for NV12), bit for bit, one fm_frame_resize launch on
+    the current stream into the next slot of a ring of `depth` device frames.
+
+    Slot reuse: a tracker resizes on the main stream at the start of a step, and every stage reads the resized frame
+    either on the main stream or on a stream that waits on an event recorded after the resize (the detector and ReID
+    streams wait on `_main_ready`).  Before the next step's resize is enqueued, the host has waited for the detector
+    stream's last event and the main stream has joined the ReID stream, so every read of a slot is ordered before the
+    next write on the main stream.  One slot would therefore do; with two, a resize never overwrites the frame the
+    previous step's stages were handed, whatever a later stage does with it."""
+
+    def __init__(self, size, depth=2, device="cuda"):
+        self._lib = _lib.load()
+        self.size = w, h = tuple(int(v) for v in size)
+        self.dev = [torch.empty((h, w, 3), dtype=torch.uint8, device=device) for _ in range(depth)]
+        self.cur = 0
+
+    def resize(self, frame):
+        """The device Frame `frame` at this resizer's size, as a BGR Frame (valid until `depth` more resizes)."""
+        out = self.dev[self.cur]
+        self.cur = (self.cur + 1) % len(self.dev)
+        _lib.check(self._lib.fm_frame_resize(C.byref(frame.fm()), ptr(out), self.size[0], self.size[1], stream_ptr()),
+                   "fm_frame_resize")
+        return Frame.bgr(out)
+
+
 def as_frame(frame, pixel_format="BGR", size=None):
     """A caller's frame as a Frame, nothing copied.  A Frame passes through; otherwise `frame` is in pixel_format:
     'BGR' -- an HxWx3 uint8 cuda tensor (contiguous) or host ndarray; 'NV12' -- any form nv12_frame accepts.  size:

@@ -16,7 +16,7 @@ import torch
 from .detector import YOLODetector, PublicDetector
 from .feature_extractor import FeatureExtractor
 from .tracker import MultiTracker
-from .devmem import FrameUploader, check_pixel_format, device_frame, prefetch_frame
+from .devmem import FrameResizer, FrameUploader, check_capture_size, check_pixel_format, device_frame, prefetch_frame
 from .utils import Profiler
 
 LOGGER = logging.getLogger(__name__)
@@ -43,14 +43,22 @@ class MOT:
                  detections_override=None,
                  embeddings_override=None,
                  embeddings_tap=None,
-                 pixel_format='BGR'):
+                 pixel_format='BGR',
+                 capture_size=None):
         """pixel_format: 'BGR' -- every frame is HxWx3 u8 (host array or cuda tensor); 'NV12' -- every frame is NV12
         as hardware video decoders emit it, in any form devmem.nv12_frame accepts (host (3H/2, W) array, pitched cuda
         tensor, or a (Y, UV) pair of cuda planes).  NV12 frames are read in place by the letterbox, crop and KLT
         kernels; tracks, detections and embeddings are those of the BGR path on cv2.cvtColor(frame,
-        cv2.COLOR_YUV2BGR_NV12)."""
+        cv2.COLOR_YUV2BGR_NV12).
+
+        size is the tracking size (the reference's resize_to).  capture_size: the (width, height) of the frames `step`
+        and `prefetch` receive (the reference's stream_cfg.resolution; even for NV12), when it differs from `size`.
+        Each frame is uploaded at that size and scaled to `size` on the GPU, bit for bit cv2.resize(frame, size) with
+        INTER_LINEAR (of the cv2 decode for NV12); tracks and boxes are in tracking-size coordinates, as in the
+        reference.  None, or capture_size == size, tracks the frames as they come."""
         self.size = size
         self.pixel_format = check_pixel_format(pixel_format)
+        self.capture_size = check_capture_size(capture_size, size, self.pixel_format)
         self.detector_type = DetectorType[detector_type.upper()]
         assert detector_frame_skip >= 1
         self.detector_frame_skip = detector_frame_skip
@@ -86,7 +94,8 @@ class MOT:
         self.tracker = MultiTracker(self.size, self.extractors[0].metric, **vars(tracker_cfg),
                                     feat_dim=self.extractors[0].feature_dim)
         self.frame_count = 0
-        self._uploader = FrameUploader(size, depth=3, pixel_format=self.pixel_format)
+        self._uploader = FrameUploader(self.capture_size, depth=3, pixel_format=self.pixel_format)
+        self._resizer = None if self.capture_size == tuple(size) else FrameResizer(size)
         self._det_stream = torch.cuda.Stream()
         self._main_ready = torch.cuda.Event()
         # ReID crops + OSNet run on their own stream so that the batched Kalman step, its read-back and the host side
@@ -128,11 +137,13 @@ class MOT:
         """Optional read-ahead: starts the host-to-device copy of the NEXT frame (the ndarray a later `step` call will
         receive) on an upload stream, so it overlaps the current step's kernels (role of the reference's VideoIO
         frame queue, fastmot/videoio.py:125-142)."""
-        prefetch_frame(frame, self._uploader, self.pixel_format, self.size)
+        prefetch_frame(frame, self._uploader, self.pixel_format, self.capture_size)
 
     def step(self, frame):
         """mot.py:125-168"""
-        frame_dev = device_frame(frame, self._uploader, self.pixel_format, self.size)
+        frame_dev = device_frame(frame, self._uploader, self.pixel_format, self.capture_size)
+        if self._resizer is not None:
+            frame_dev = self._resizer.resize(frame_dev)    # on the main stream, before _main_ready is recorded
         detections = []
         if self.frame_count == 0:
             self._detect_async(frame_dev)

@@ -21,7 +21,7 @@ import torch
 from .detector import YOLODetector
 from .feature_extractor import FeatureExtractor
 from .tracker import MultiTracker
-from .devmem import FrameUploader, check_pixel_format, device_frame, prefetch_frame
+from .devmem import FrameResizer, FrameUploader, check_capture_size, check_pixel_format, device_frame, prefetch_frame
 from .mot import DetectorType
 from .utils import Profiler
 
@@ -58,13 +58,19 @@ class MultiCameraMOT:
                  draw=False,
                  detections_override=None,
                  embeddings_override=None,
-                 pixel_format='BGR'):
-        """sizes: one (width, height) per camera.  pixel_format ('BGR' or 'NV12', as in MOT) applies to every
-        camera of the group.  The keyword arguments are MOT's, so the reference's `mot_cfg`
+                 pixel_format='BGR',
+                 capture_size=None,
+                 capture_sizes=None):
+        """sizes: one (width, height) tracking size per camera.  pixel_format ('BGR' or 'NV12', as in MOT) applies to
+        every camera of the group.  The keyword arguments are MOT's, so the reference's `mot_cfg`
         (cfg/mot.json) passes unchanged; ssd_detector_cfg, public_detector_cfg and visualizer_cfg are accepted and
         unused, since only the YOLO detector runs several cameras.  detections_override(camera, frame_id) and
         embeddings_override(camera, frame_id, detections) replace the networks' OUTPUT after both ran, as MOT's hooks
-        do; frame_id is the camera's local frame count."""
+        do; frame_id is the camera's local frame count.
+
+        capture_sizes: one entry per camera, the (width, height) its frames arrive at, or None for a camera whose
+        frames come at its tracking size; a scaled camera's frames are resized on the GPU as MOT(capture_size=...)
+        resizes them.  capture_size: one capture size for every camera (MOT's keyword); give at most one of the two."""
         if len(sizes) < 1:
             raise ValueError("MultiCameraMOT needs at least one camera")
         self.sizes = []
@@ -74,6 +80,18 @@ class MultiCameraMOT:
             self.sizes.append(tuple(int(v) for v in wh))
         self.num_cameras = N = len(self.sizes)
         self.pixel_format = check_pixel_format(pixel_format)
+        if capture_size is not None and capture_sizes is not None:
+            raise ValueError("give capture_size (every camera) or capture_sizes (one per camera), not both")
+        if capture_sizes is None:
+            capture_sizes = [capture_size] * N
+        if len(capture_sizes) != N:
+            raise ValueError(f"capture_sizes: expected {N} entries (one per camera), got {len(capture_sizes)}")
+        self.capture_sizes = []
+        for s, (cs, wh) in enumerate(zip(capture_sizes, self.sizes)):
+            try:
+                self.capture_sizes.append(check_capture_size(cs, wh, self.pixel_format))
+            except ValueError as e:
+                raise ValueError(f"camera {s}: {e}") from None
         self.detector_type = DetectorType[detector_type.upper()]
         if self.detector_type != DetectorType.YOLO:
             raise NotImplementedError(f"detector_type {detector_type!r}: several cameras are tracked with the batched "
@@ -106,7 +124,8 @@ class MultiCameraMOT:
         self.trackers = [MultiTracker(wh, self.extractors[0].metric, **vars(tracker_cfg),
                                       feat_dim=self.extractors[0].feature_dim) for wh in self.sizes]
         self.frame_counts = [0] * N
-        self._uploaders = [FrameUploader(wh, depth=3, pixel_format=self.pixel_format) for wh in self.sizes]
+        self._uploaders = [FrameUploader(wh, depth=3, pixel_format=self.pixel_format) for wh in self.capture_sizes]
+        self._resizers = [None if cs == wh else FrameResizer(wh) for cs, wh in zip(self.capture_sizes, self.sizes)]
         self._det_stream = torch.cuda.Stream()
         self._main_ready = torch.cuda.Event()
         self._reid_stream = torch.cuda.Stream()
@@ -134,12 +153,12 @@ class MultiCameraMOT:
         self._each_frame(prefetch_frame, frames)
 
     def _each_frame(self, fn, frames):
-        """[fn(frame, camera's uploader, pixel format, camera's size) or None] over the cameras' frames (None: no
-        frame); a frame of the wrong size or form raises ValueError naming its camera."""
+        """[fn(frame, camera's uploader, pixel format, camera's capture size) or None] over the cameras' frames (None:
+        no frame); a frame of the wrong size or form raises ValueError naming its camera."""
         if len(frames) != self.num_cameras:
             raise ValueError(f"expected {self.num_cameras} frames, got {len(frames)}")
         out = []
-        for s, (f, up, wh) in enumerate(zip(frames, self._uploaders, self.sizes)):
+        for s, (f, up, wh) in enumerate(zip(frames, self._uploaders, self.capture_sizes)):
             try:
                 out.append(None if f is None else fn(f, up, self.pixel_format, wh))
             except ValueError as e:
@@ -162,6 +181,8 @@ class MultiCameraMOT:
         """One step of the group: frames[s] is camera s's next frame in the group's pixel format (HxWx3 u8 host array
         or cuda tensor; NV12 in any form MOT takes), or None when camera s has no frame on this step."""
         frames_dev = self._each_frame(device_frame, frames)
+        # scaled cameras: resized on the main stream, before _main_ready is recorded (devmem.FrameResizer)
+        frames_dev = [f if f is None or r is None else r.resize(f) for f, r in zip(frames_dev, self._resizers)]
         init, detect, track = plan_step(self.frame_counts, [f is not None for f in frames], self.detector_frame_skip)
         cams = sorted(init + detect)                 # the detector batch, in camera order
         if not cams:

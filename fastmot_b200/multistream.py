@@ -25,13 +25,15 @@ class MultiStreamMOT(MultiCameraMOT):
                  draw=False,
                  detections_override=None,
                  embeddings_override=None,
-                 pixel_format='BGR'):
+                 pixel_format='BGR',
+                 capture_size=None):
         """size: (width, height) shared by every stream; pixel_format ('BGR' or 'NV12', as in MOT) applies to every
         stream.  The keyword arguments are MOT's, so the reference's
         `mot_cfg` (cfg/mot.json) passes unchanged; ssd_detector_cfg, public_detector_cfg and visualizer_cfg are
         accepted and unused, since only the YOLO detector runs several streams.  detections_override(stream,
         frame_id) and embeddings_override(stream, frame_id, detections) replace the networks' OUTPUT after both ran,
-        as MOT's hooks do."""
+        as MOT's hooks do.  capture_size: the (width, height) every stream's frames arrive at when it differs from
+        `size`, as in MOT; each frame is resized to `size` on the GPU."""
         if not (isinstance(size, (tuple, list)) and len(size) == 2 and all(np.isscalar(v) for v in size)):
             raise ValueError("MultiStreamMOT takes one frame size (width, height) shared by every stream; "
                              "streams of different sizes need MultiCameraMOT")
@@ -45,7 +47,7 @@ class MultiStreamMOT(MultiCameraMOT):
                          public_detector_cfg=public_detector_cfg, feature_extractor_cfgs=feature_extractor_cfgs,
                          tracker_cfg=tracker_cfg, visualizer_cfg=visualizer_cfg, draw=draw,
                          detections_override=detections_override, embeddings_override=embeddings_override,
-                         pixel_format=pixel_format)
+                         pixel_format=pixel_format, capture_size=capture_size)
 
     @property
     def frame_count(self):

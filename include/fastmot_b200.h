@@ -221,6 +221,14 @@ int fm_roi_resize_norm(const FmFrame* frame, const double* tlbrs, const int* n_d
 int fm_roi_resize_norm_geom(const FmFrameGeom* geom, const int* frame_idx, const double* tlbrs, int n, int out_w,
                             int out_h, int layout, void* out, void* stream);
 
+/* cv2.resize(bgr(src), (dw, dh)) with the default INTER_LINEAR into a tight dh x dw x 3 u8 BGR frame.  bgr(src) is
+ * src itself for FM_PIX_BGR, cv2.cvtColor(src, COLOR_YUV2BGR_NV12) for FM_PIX_NV12 (read in place, as the letterbox
+ * / crop / gray kernels read it).  dst must not overlap src.  Bit-identical to OpenCV 4.13: an exact 2x downscale in
+ * both axes is the 2x2 rounded mean, every other size pair the 11-bit fixed-point generic path.  Any size pair is
+ * accepted (dh <= 65535); capture frames tracked at another size go through it (a camera's stream_cfg.resolution ->
+ * resize_to). */
+int fm_frame_resize(const FmFrame* src, unsigned char* dst, int dw, int dh, void* stream);
+
 /* CalDetection / CalDetection_NewCoords (fastmot/plugins/yolo_layer.cu:127-230) fused with the class mask +
  * score threshold + pixel scaling of YOLODetector._filter_dets (fastmot/detector.py:331-341).  One call per
  * head; head_out is [(5+C)*A, H, W] (nhwc = 0, the plugin's layout) or [H, W, (5+C)*A] (nhwc = 1), fp32 or fp16.  Survivors write their 7-float record to
