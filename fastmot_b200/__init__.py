@@ -9,7 +9,7 @@ from .tracker import MultiTracker, DeviceEmbeddings
 from .detector import YOLODetector, PublicDetector, DET_DTYPE
 from .feature_extractor import FeatureExtractor
 from .mot import MOT
-from .devmem import Frame, nv12_frame
+from .devmem import Frame, nv12_frame, pixel_frame
 from .multicamera import MultiCameraMOT
 from .multistream import MultiStreamMOT
 from . import models

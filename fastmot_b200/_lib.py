@@ -80,7 +80,8 @@ class FmYoloHead(C.Structure):
 
 
 class FmFrame(C.Structure):
-    _fields_ = [("y", c_p), ("uv", c_p), ("w", c_i), ("h", c_i), ("pitch", c_i), ("uv_pitch", c_i), ("format", c_i)]
+    _fields_ = [("y", c_p), ("uv", c_p), ("w", c_i), ("h", c_i), ("pitch", c_i), ("uv_pitch", c_i), ("format", c_i),
+                ("v", c_p)]
 
 
 class FmFrameGeom(C.Structure):
@@ -88,7 +89,7 @@ class FmFrameGeom(C.Structure):
                 ("size_w", c_f), ("size_h", c_f), ("off_x", c_f), ("off_y", c_f)]
 
 
-FM_PIX_BGR, FM_PIX_NV12 = 0, 1
+FM_PIX_BGR, FM_PIX_NV12, FM_PIX_I420, FM_PIX_YUY2, FM_PIX_BGRX = 0, 1, 2, 3, 4
 
 
 # name -> (restype, argtypes); kept in one table so tests can check it against the header

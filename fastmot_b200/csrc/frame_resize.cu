@@ -1,7 +1,7 @@
 // Frame resize (HBM-bound, one pass): cv2.resize(frame, (dw, dh)) with the default INTER_LINEAR into a tight BGR u8
-// frame, for cameras that capture at another size than the one they are tracked at.  A BGR or an NV12 frame (FmFrame)
-// is read in place; each NV12 tap is converted to BGR before it is interpolated (pixel_src.cuh), so the result is
-// cv2.resize of cv2.cvtColor(frame, COLOR_YUV2BGR_NV12).
+// frame, for cameras that capture at another size than the one they are tracked at.  A frame of any pixel format
+// (FmFrame) is read in place; each YUV tap is converted to BGR before it is interpolated (pixel_src.cuh), so the result
+// is cv2.resize of the frame's cv2.cvtColor decode.
 //   * exactly 2x smaller in both axes: OpenCV takes its 2x2 area path, (a + b + c + d + 2) >> 2 per channel;
 //   * any other size pair: the generic 11-bit fixed-point path of cv_linear.cuh (an exact 3x is NOT special-cased).
 // One thread per output pixel; the three bytes of consecutive pixels are consecutive, so a warp stores 96 contiguous

@@ -1,6 +1,6 @@
 // KLT image pyramid kernels (byte work, HBM/L2-bound): BGR->gray + 0.5x box mean in one pass, BGR->gray + an
-// INTER_LINEAR resize to any optical-flow size (both also reading NV12 frames in place, pixel_src.cuh), 5-tap Gaussian
-// pyrDown, int16 Scharr derivatives, 0.1x background image + mask.
+// INTER_LINEAR resize to any optical-flow size (both also reading YUV and BGRx frames in place, pixel_src.cuh),
+// 5-tap Gaussian pyrDown, int16 Scharr derivatives, 0.1x background image + mask.
 //
 // Reference: fastmot/flow.py:121-133, 153-154, 187-189 (cv2.cvtColor / cv2.resize) and the pyramid that
 // cv2.calcOpticalFlowPyrLK builds internally (flow.py:203-207; OpenCV lkpyramid.cpp: buildOpticalFlowPyramid,
@@ -19,20 +19,31 @@ __device__ __forceinline__ int gray_of(const int p[3]) {
 }
 
 // The four pixels of the 2x2 block at (x0, y0) (x1 = x0 + 1, y1 = y0 + 1 inside the frame; w and h are even).
-__device__ __forceinline__ void block_bgr(const BgrSrc& s, int x0, int y0, int x1, int y1, int a[3], int b[3],
-                                          int c[3], int d[3]) {
+template <class Src>
+__device__ __forceinline__ void block_bgr(const Src& s, int x0, int y0, int x1, int y1, int a[3], int b[3], int c[3],
+                                          int d[3]) {
     s.px(x0, y0, a); s.px(x1, y0, b); s.px(x0, y1, c); s.px(x1, y1, d);
 }
 
-// An NV12 2x2 block at even (x0, y0) is exactly one chroma sample: one UV load for the four pixels.
-__device__ __forceinline__ void block_bgr(const Nv12Src& s, int x0, int y0, int x1, int y1, int a[3], int b[3],
-                                          int c[3], int d[3]) {
-    const unsigned char* q = s.uv + (size_t)(y0 >> 1) * s.uv_pitch + x0;
-    const int U = q[0], V = q[1];
+// A 4:2:0 2x2 block at even (x0, y0) is exactly one chroma sample: one U and one V load for the four pixels.
+template <int CSTEP>
+__device__ __forceinline__ void block_bgr(const Yuv420Src<CSTEP>& s, int x0, int y0, int x1, int y1, int a[3],
+                                          int b[3], int c[3], int d[3]) {
+    const size_t q = s.chroma(x0, y0);
+    const int U = s.U(q), V = s.V(q);
     const unsigned char* r0 = s.y + (size_t)y0 * s.y_pitch;
     const unsigned char* r1 = s.y + (size_t)y1 * s.y_pitch;
     fm_yuv_to_bgr(r0[x0], U, V, a); fm_yuv_to_bgr(r0[x1], U, V, b);
     fm_yuv_to_bgr(r1[x0], U, V, c); fm_yuv_to_bgr(r1[x1], U, V, d);
+}
+
+// A YUY2 2x2 block at even (x0, y0) is one pixel pair per row: one Y0 U Y1 V group each.
+__device__ __forceinline__ void block_bgr(const Yuy2Src& s, int x0, int y0, int x1, int y1, int a[3], int b[3],
+                                          int c[3], int d[3]) {
+    const unsigned char* q0 = s.p + (size_t)y0 * s.pitch + x0 * 2;
+    const unsigned char* q1 = s.p + (size_t)y1 * s.pitch + x0 * 2;
+    fm_yuv_to_bgr(q0[0], q0[1], q0[3], a); fm_yuv_to_bgr(q0[2], q0[1], q0[3], b);
+    fm_yuv_to_bgr(q1[0], q1[1], q1[3], c); fm_yuv_to_bgr(q1[2], q1[1], q1[3], d);
 }
 
 // One thread per 2x2 block of the full-resolution frame.

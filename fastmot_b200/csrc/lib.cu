@@ -12,7 +12,7 @@ extern "C" void fm_set_last_error(const char* msg) {
 
 extern "C" const char* fm_last_error(void) { return g_last_error; }
 
-extern "C" int fm_version(void) { return 102; }
+extern "C" int fm_version(void) { return 103; }
 
 extern "C" int fm_device_ok(void) {
     int n = 0;

@@ -4,7 +4,7 @@
 //   fm_roi_resize_norm   : per-detection crop + OpenCV-style fixed-point bilinear resize to 128x256 + ImageNet
 //                          normalisation, all crops in one launch (fastmot/feature_extractor.py:48-60, 84-98;
 //                          fastmot/utils/rect.py:92-97)
-// Both read a BGR or an NV12 frame (FmFrame) in place; an NV12 bilinear tap is converted to BGR before it is
+// Both read a frame of any pixel format (FmFrame) in place; a YUV bilinear tap is converted to BGR before it is
 // interpolated (pixel_src.cuh).  The *_geom entries read each frame (and, for the letterbox, its ROI) from a device
 // FmFrameGeom table (one grid slice per frame, or one frame index per crop), so one launch covers several frames of
 // any sizes and formats; every pixel is computed by the same body as in the one-frame entries.
@@ -57,7 +57,7 @@ __device__ __forceinline__ void letterbox_px(const Src& src, int src_w, int src_
     const int x0 = (int)floor(sx), y0 = (int)floor(sy);
     const int x1 = min(x0 + 1, src_w - 1), y1 = min(y0 + 1, src_h - 1);
     const double fx = sx - x0, fy = sy - y0;
-    // each tap is a BGR pixel before interpolation (an NV12 tap is converted with its own chroma)
+    // each tap is a BGR pixel before interpolation (a YUV tap is converted with its own chroma)
     int p00[3], p01[3], p10[3], p11[3];
     src.px(x0, y0, p00);
     src.px(x1, y0, p01);
@@ -82,7 +82,7 @@ __global__ void __launch_bounds__(256) letterbox_kernel(Src src, int src_w, int 
     letterbox_px<LAYOUT>(src, src_w, src_h, dst_w, dst_h, roi_x, roi_y, roi_w, roi_h, out, x, blockIdx.y);
 }
 
-// image blockIdx.z takes its frame (BGR or NV12), size and ROI from geom[blockIdx.z] and writes the blockIdx.z-th
+// image blockIdx.z takes its frame (any pixel format), size and ROI from geom[blockIdx.z] and writes the blockIdx.z-th
 // NHWC8 image of out
 __global__ void __launch_bounds__(256) letterbox_geom_kernel(const FmFrameGeom* __restrict__ geom, int dst_w,
                                                               int dst_h, void* __restrict__ out) {
@@ -123,7 +123,7 @@ __device__ __forceinline__ void roi_px(const Src& src, int src_w, int src_h, con
     cv_coef(x, (double)cw / out_w, cw, sx, a0, a1);
     cv_coef(y, (double)ch / out_h, ch, sy, b0, b1);
     const int sx1 = min(sx + 1, cw - 1), sy1 = min(sy + 1, ch - 1);
-    // each tap is a BGR pixel before interpolation (an NV12 tap is converted with its own chroma)
+    // each tap is a BGR pixel before interpolation (a YUV tap is converted with its own chroma)
     int p00[3], p01[3], p10[3], p11[3];
     src.px(cx0 + sx, cy0 + sy, p00);
     src.px(cx0 + sx1, cy0 + sy, p01);
@@ -159,7 +159,7 @@ __global__ void __launch_bounds__(128) roi_resize_norm_kernel(Src src, int src_w
     roi_px<LAYOUT>(src, src_w, src_h, tlbrs, crop, out_w, out_h, out, x, blockIdx.y);
 }
 
-// crop i is cut from geom[frame_idx[i]]'s frame (BGR or NV12), with that frame's own width and height
+// crop i is cut from geom[frame_idx[i]]'s frame (any pixel format), with that frame's own width and height
 template <int LAYOUT>
 __global__ void __launch_bounds__(128) roi_resize_norm_geom_kernel(const FmFrameGeom* __restrict__ geom,
                                                                     const int* __restrict__ frame_idx,

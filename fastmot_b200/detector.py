@@ -157,7 +157,7 @@ class YOLODetector(Detector):
     # ------------------------------------------------------------------
     def preprocess(self, frame_dev):
         """fastmot/detector.py:289-300 on the device (frame_dev: HxWx3 u8 cuda tensor, or a device Frame of this
-        detector's size: an NV12 frame is read in place)."""
+        detector's size: a frame of any pixel format is read in place)."""
         f = device_frame(frame_dev, size=self.size)
         rx, ry, rw, rh = self.roi
         rc = self._lib.fm_letterbox_preproc(C.byref(f.fm()), self.input_wh[0], self.input_wh[1], rx, ry, rw, rh, 1,
@@ -165,7 +165,7 @@ class YOLODetector(Detector):
         _lib.check(rc, "fm_letterbox_preproc")
 
     def detect_async(self, frame):
-        """Upload (if `frame` is a host array or a host NV12 Frame), pre-process, run the conv stack and the whole
+        """Upload (if `frame` is a host array or a host Frame), pre-process, run the conv stack and the whole
         post-processing asynchronously; `postprocess` waits for the D result rows."""
         self.frame_dev = device_frame(frame, self._uploads[0])
         self.preprocess(self.frame_dev)

@@ -105,15 +105,29 @@ class Downlink:
         return out
 
 
-PIXEL_FORMATS = ("BGR", "NV12")
+class _PixelFormat:
+    """One row of the pixel-format table: the FmFrame format code, the shape of a host frame of size (w, h), whether
+    the width and the height must be even, and the parser of the frame forms the format accepts."""
+    __slots__ = ("code", "shape", "even_w", "even_h", "layout")
+
+    def __init__(self, code, shape, even_w, even_h, layout):
+        self.code, self.shape, self.even_w, self.even_h, self.layout = code, shape, even_w, even_h, layout
 
 
 def check_pixel_format(pixel_format):
-    """'BGR' or 'NV12' (any case) -> the upper-case name; anything else raises ValueError."""
+    """One of PIXEL_FORMATS (any case) -> the upper-case name; anything else raises ValueError."""
     fmt = str(pixel_format).upper()
     if fmt not in PIXEL_FORMATS:
         raise ValueError(f"pixel_format must be one of {PIXEL_FORMATS}, got {pixel_format!r}")
     return fmt
+
+
+def _check_size(fmt, w, h):
+    """Raises ValueError unless (w, h) is a frame size `fmt` can have."""
+    p = _FORMATS[fmt]
+    if w < 1 or h < 1 or (p.even_w and w % 2) or (p.even_h and h % 2):
+        need = ("an even width and height" if p.even_h else "an even width") if p.even_w else "a non-empty size"
+        raise ValueError(f"{fmt} needs {need}, got {w}x{h}")
 
 
 class Frame:
@@ -121,15 +135,19 @@ class Frame:
 
     BGR: `y` is an HxWx3 uint8 cuda tensor (tight rows); `uv` is None.
     NV12 (hardware video decoders): `y` is the H x W luma plane and `uv` the H/2 x W plane of interleaved U, V at half
-    resolution, each with its own row pitch in bytes (`y_pitch`, `uv_pitch` >= W).  Build NV12 frames with
-    `nv12_frame`; the planes are views of the caller's memory, nothing is copied.
-    A host frame (`on_device` False) holds its ndarray in `y` (HxWx3 BGR or (3H/2, W) NV12); `device_frame` uploads it.
+    resolution, each with its own row pitch in bytes (`y_pitch`, `uv_pitch` >= W).
+    I420 (software decoders): `y` is the H x W luma plane, `uv` the H/2 x W/2 U plane and `v` the V plane, U and V
+    with one row pitch `uv_pitch` >= W/2.
+    YUY2 (USB cameras) and BGRX (nvvidconv): `y` is the H x W x 2 or H x W x 4 packed plane, row pitch `y_pitch`.
+    Build them with `pixel_frame` (or `nv12_frame`); the planes are views of the caller's memory, nothing is copied.
+    A host frame (`on_device` False) holds its ndarray in `y` (the host shape of its format, FrameUploader.frame_shape);
+    `device_frame` uploads it.
     """
-    __slots__ = ("format", "w", "h", "y", "uv", "y_pitch", "uv_pitch", "_fm")
+    __slots__ = ("format", "w", "h", "y", "uv", "y_pitch", "uv_pitch", "v", "_fm")
 
-    def __init__(self, format, w, h, y, uv=None, y_pitch=0, uv_pitch=0):
+    def __init__(self, format, w, h, y, uv=None, y_pitch=0, uv_pitch=0, v=None):
         self.format, self.w, self.h = format, int(w), int(h)
-        self.y, self.uv, self.y_pitch, self.uv_pitch = y, uv, int(y_pitch), int(uv_pitch)
+        self.y, self.uv, self.y_pitch, self.uv_pitch, self.v = y, uv, int(y_pitch), int(uv_pitch), v
         self._fm = None
 
     @classmethod
@@ -152,37 +170,50 @@ class Frame:
         """The FmFrame of this device frame, which every C entry point that reads camera pixels takes (built on the
         first call).  It holds raw plane addresses: keep this Frame referenced until the kernels that read them ran."""
         if self._fm is None:
-            nv12 = self.format == "NV12"
-            self._fm = _lib.FmFrame(self.y.data_ptr(), self.uv.data_ptr() if nv12 else None, self.w, self.h,
-                                    self.y_pitch, self.uv_pitch, _lib.FM_PIX_NV12 if nv12 else _lib.FM_PIX_BGR)
+            addr = lambda t: None if t is None else t.data_ptr()
+            self._fm = _lib.FmFrame(self.y.data_ptr(), addr(self.uv), self.w, self.h, self.y_pitch, self.uv_pitch,
+                                    _FORMATS[self.format].code, addr(self.v))
         return self._fm
 
 
-def _plane(t, rows, w, what):
-    """Checks one NV12 plane: a 2-D uint8 tensor of `rows` x w with unit column stride and any row stride >= w."""
+def _plane(t, rows, cols, what):
+    """Checks one plane: a 2-D uint8 tensor of rows x cols with unit column stride and any row stride >= cols."""
     if not torch.is_tensor(t):
-        raise ValueError(f"NV12 {what}: expected a uint8 cuda tensor, got {type(t).__name__}")
+        raise ValueError(f"{what}: expected a uint8 cuda tensor, got {type(t).__name__}")
     if t.dtype != torch.uint8 or t.dim() != 2:
-        raise ValueError(f"NV12 {what}: expected a 2-D uint8 tensor, got {t.dtype} of shape {tuple(t.shape)}")
-    if tuple(t.shape) != (rows, w):
-        raise ValueError(f"NV12 {what}: expected shape {(rows, w)}, got {tuple(t.shape)}")
-    if t.stride(1) != 1 or t.stride(0) < w:
-        raise ValueError(f"NV12 {what}: expected stride(1) == 1 and stride(0) >= {w} (the width), got strides "
+        raise ValueError(f"{what}: expected a 2-D uint8 tensor, got {t.dtype} of shape {tuple(t.shape)}")
+    if tuple(t.shape) != (rows, cols):
+        raise ValueError(f"{what}: expected shape {(rows, cols)}, got {tuple(t.shape)}")
+    if t.stride(1) != 1 or t.stride(0) < cols:
+        raise ValueError(f"{what}: expected stride(1) == 1 and stride(0) >= {cols} (the row length), got strides "
                          f"{tuple(t.stride())}")
 
 
-def _even(w, h):
-    if w < 2 or h < 2 or w % 2 or h % 2:
-        raise ValueError(f"NV12 needs an even width and height, got {w}x{h}")
+def _is_u8(a):
+    return a.dtype == (torch.uint8 if torch.is_tensor(a) else np.uint8)
 
 
-def nv12_layout(frame):
-    """Checks the shape, dtype and strides of an NV12 frame in one of the forms `nv12_frame` takes and returns its
-    Frame, without looking at the device its tensors live on."""
-    if isinstance(frame, Frame):
-        if frame.format != "NV12":
-            raise ValueError(f"expected an NV12 frame, got a {frame.format} Frame")
-        return frame
+def _yuv420_size(fmt, frame):
+    """(w, h) of a (3H/2, W) uint8 4:2:0 frame (ndarray or tensor), checked."""
+    if not _is_u8(frame) or frame.ndim != 2 or frame.shape[0] % 3:
+        kind = "ndarray" if isinstance(frame, np.ndarray) else "cuda tensor"
+        raise ValueError(f"{fmt} frame: expected a (3H/2, W) uint8 {kind}, got {frame.dtype} of shape "
+                         f"{tuple(frame.shape)}")
+    w, h = int(frame.shape[1]), int(frame.shape[0]) * 2 // 3
+    _check_size(fmt, w, h)
+    return w, h
+
+
+def _bgr_layout(frame):
+    if torch.is_tensor(frame):
+        return Frame.bgr(frame)
+    if not (isinstance(frame, np.ndarray) and frame.dtype == np.uint8 and frame.ndim == 3 and frame.shape[2] == 3):
+        raise ValueError(f"BGR host frame: expected an HxWx3 uint8 ndarray, got {type(frame).__name__} "
+                         f"{getattr(frame, 'dtype', '')} {getattr(frame, 'shape', '')}")
+    return Frame("BGR", frame.shape[1], frame.shape[0], frame)
+
+
+def _nv12_layout(frame):
     if isinstance(frame, (tuple, list)):
         if len(frame) != 2:
             raise ValueError(f"NV12 planes: expected a pair (Y (H, W), UV (H/2, W)), got {len(frame)} items")
@@ -190,26 +221,124 @@ def nv12_layout(frame):
         if not torch.is_tensor(y) or y.dim() != 2:
             raise ValueError("NV12 Y plane: expected a 2-D uint8 cuda tensor (H, W)")
         h, w = y.shape
-        _even(w, h)
-        _plane(y, h, w, "Y plane")
-        _plane(uv, h // 2, w, "UV plane")
+        _check_size("NV12", w, h)
+        _plane(y, h, w, "NV12 Y plane")
+        _plane(uv, h // 2, w, "NV12 UV plane")
         return Frame("NV12", w, h, y, uv, y.stride(0), uv.stride(0))
     if isinstance(frame, np.ndarray):
-        if frame.dtype != np.uint8 or frame.ndim != 2 or frame.shape[0] % 3:
-            raise ValueError(f"NV12 host frame: expected a (3H/2, W) uint8 ndarray, got {frame.dtype} of shape "
-                             f"{frame.shape}")
-        h, w = frame.shape[0] * 2 // 3, frame.shape[1]
-        _even(w, h)
+        w, h = _yuv420_size("NV12", frame)
         return Frame("NV12", w, h, frame)
     if torch.is_tensor(frame):
-        if frame.dim() != 2 or frame.shape[0] % 3:
-            raise ValueError(f"NV12 frame: expected a (3H/2, W) uint8 cuda tensor, got shape {tuple(frame.shape)}")
-        h, w = frame.shape[0] * 2 // 3, frame.shape[1]
-        _even(w, h)
-        _plane(frame, 3 * h // 2, w, "frame")
+        w, h = _yuv420_size("NV12", frame)
+        _plane(frame, 3 * h // 2, w, "NV12 frame")
         return Frame("NV12", w, h, frame[:h], frame[h:], frame.stride(0), frame.stride(0))
     raise ValueError(f"NV12 frame: expected a (3H/2, W) uint8 ndarray or cuda tensor, or a (Y, UV) pair of cuda "
                      f"tensors, got {type(frame).__name__}")
+
+
+def _i420_layout(frame):
+    if isinstance(frame, (tuple, list)):
+        if len(frame) != 3:
+            raise ValueError(f"I420 planes: expected a triple (Y (H, W), U (H/2, W/2), V (H/2, W/2)), got "
+                             f"{len(frame)} items")
+        y, u, v = frame
+        if not torch.is_tensor(y) or y.dim() != 2:
+            raise ValueError("I420 Y plane: expected a 2-D uint8 cuda tensor (H, W)")
+        h, w = y.shape
+        _check_size("I420", w, h)
+        _plane(y, h, w, "I420 Y plane")
+        _plane(u, h // 2, w // 2, "I420 U plane")
+        _plane(v, h // 2, w // 2, "I420 V plane")
+        if u.stride(0) != v.stride(0):
+            raise ValueError(f"I420 U and V planes: expected equal row strides, got {u.stride(0)} and {v.stride(0)}")
+        return Frame("I420", w, h, y, u, y.stride(0), u.stride(0), v)
+    if isinstance(frame, np.ndarray):
+        w, h = _yuv420_size("I420", frame)
+        return Frame("I420", w, h, frame)
+    if torch.is_tensor(frame):
+        w, h = _yuv420_size("I420", frame)
+        if not frame.is_contiguous():
+            raise ValueError(f"I420 frame: expected a tight (3H/2, W) tensor (strides ({w}, 1)), got strides "
+                             f"{tuple(frame.stride())}; give pitched planes as a (Y, U, V) triple")
+        q = h * w // 4
+        chroma = frame[h:].reshape(-1)
+        u, v = chroma[:q].view(h // 2, w // 2), chroma[q:].view(h // 2, w // 2)
+        return Frame("I420", w, h, frame[:h], u, w, w // 2, v)
+    raise ValueError(f"I420 frame: expected a (3H/2, W) uint8 ndarray or cuda tensor, or a (Y, U, V) triple of cuda "
+                     f"tensors, got {type(frame).__name__}")
+
+
+def _packed_layout(fmt, ch):
+    """The parser of a packed format of `ch` bytes per pixel: a host (H, W, ch) uint8 ndarray, or a cuda tensor of that
+    shape with strides (>= ch W, ch, 1) (rows may be pitched)."""
+    form = f"(H, W, {ch}) uint8"
+
+    def layout(frame):
+        if isinstance(frame, np.ndarray) or torch.is_tensor(frame):
+            kind = "ndarray" if isinstance(frame, np.ndarray) else "cuda tensor"
+            if not _is_u8(frame) or frame.ndim != 3 or frame.shape[2] != ch:
+                raise ValueError(f"{fmt} frame: expected an {form} {kind}, got {frame.dtype} of shape "
+                                 f"{tuple(frame.shape)}")
+            h, w = int(frame.shape[0]), int(frame.shape[1])
+            _check_size(fmt, w, h)
+            if isinstance(frame, np.ndarray):
+                return Frame(fmt, w, h, frame)
+            if frame.stride(2) != 1 or frame.stride(1) != ch or frame.stride(0) < ch * w:
+                raise ValueError(f"{fmt} frame: expected strides (>= {ch * w}, {ch}, 1), got {tuple(frame.stride())}")
+            return Frame(fmt, w, h, frame, y_pitch=frame.stride(0))
+        raise ValueError(f"{fmt} frame: expected an {form} ndarray or cuda tensor, got {type(frame).__name__}")
+    return layout
+
+
+# The one table of pixel formats: every other place asks it.
+_FORMATS = {
+    "BGR": _PixelFormat(_lib.FM_PIX_BGR, lambda w, h: (h, w, 3), False, False, _bgr_layout),
+    "NV12": _PixelFormat(_lib.FM_PIX_NV12, lambda w, h: (3 * h // 2, w), True, True, _nv12_layout),
+    "I420": _PixelFormat(_lib.FM_PIX_I420, lambda w, h: (3 * h // 2, w), True, True, _i420_layout),
+    "YUY2": _PixelFormat(_lib.FM_PIX_YUY2, lambda w, h: (h, w, 2), True, False, _packed_layout("YUY2", 2)),
+    "BGRX": _PixelFormat(_lib.FM_PIX_BGRX, lambda w, h: (h, w, 4), False, False, _packed_layout("BGRX", 4)),
+}
+PIXEL_FORMATS = tuple(_FORMATS)
+
+
+def frame_layout(frame, pixel_format):
+    """Checks the shape, dtype and strides of a frame in one of the forms `pixel_frame` takes for `pixel_format` and
+    returns its Frame, without looking at the device its tensors live on.  A Frame of that format passes through."""
+    fmt = check_pixel_format(pixel_format)
+    if isinstance(frame, Frame):
+        if frame.format != fmt:
+            raise ValueError(f"expected a {fmt} frame, got a {frame.format} Frame")
+        return frame
+    return _FORMATS[fmt].layout(frame)
+
+
+def pixel_frame(frame, pixel_format):
+    """The Frame of a frame in `pixel_format`, given as
+      - BGR : a host ndarray (H, W, 3) uint8, or a contiguous cuda tensor of that shape;
+      - NV12: any form `nv12_frame` takes;
+      - I420: a host ndarray (3H/2, W) uint8 (Y rows, then the U and the V plane: cv2's layout), a tight cuda tensor
+        (3H/2, W), or a triple (Y, U, V) of cuda tensors (H, W), (H/2, W/2), (H/2, W/2) with unit column stride, any
+        Y row stride >= W and one U / V row stride >= W/2;
+      - YUY2: a host ndarray (H, W, 2) uint8 (Y0 U Y1 V per pixel pair: cv2's layout), or a cuda tensor of that shape
+        with strides (>= 2W, 2, 1); W even;
+      - BGRX: a host ndarray (H, W, 4) uint8, or a cuda tensor of that shape with strides (>= 4W, 4, 1).
+    NV12 and I420 need an even width and height.  A Frame of that format passes through.  Anything else (wrong shape,
+    dtype or device, odd size, row stride too small) raises ValueError naming what was expected."""
+    f = frame_layout(frame, pixel_format)
+    if f.on_device:
+        planes = [t for t in (f.y, f.uv, f.v) if t is not None]
+        if not all(t.is_cuda for t in planes):
+            raise ValueError(f"{f.format} frame: expected cuda tensors, got tensors on "
+                             f"{' and '.join(str(t.device) for t in planes)} (host frames are uint8 ndarrays)")
+        if len({t.device for t in planes}) > 1:
+            raise ValueError(f"{f.format} planes on different devices: "
+                             f"{' and '.join(str(t.device) for t in planes)}")
+    return f
+
+
+def nv12_layout(frame):
+    """frame_layout(frame, 'NV12')."""
+    return frame_layout(frame, "NV12")
 
 
 def nv12_frame(frame):
@@ -220,19 +349,13 @@ def nv12_frame(frame):
         plane does not follow row H, e.g. 1080p decoded into 1088-row surfaces).
     A Frame passes through.  Anything else (wrong shape, dtype or device, odd size, row stride below W) raises
     ValueError naming what was expected."""
-    f = nv12_layout(frame)
-    if f.on_device:
-        if not f.y.is_cuda or not f.uv.is_cuda:
-            raise ValueError(f"NV12 frame: expected cuda tensors, got tensors on {f.y.device} and {f.uv.device} "
-                             "(host frames are (3H/2, W) uint8 ndarrays)")
-        if f.y.device != f.uv.device:
-            raise ValueError(f"NV12 planes on different devices: {f.y.device} and {f.uv.device}")
-    return f
+    return pixel_frame(frame, "NV12")
 
 
 class FrameUploader:
-    """Host frame -> device tensor with one async copy: HxWx3 u8 BGR frames, or (pixel_format 'NV12') (3H/2, W) u8
-    NV12 frames, which move half the bytes.  Page-locked sources (detected with cudaPointerGetAttributes) are copied
+    """Host frame -> device tensor with one async copy, of the host shape of `pixel_format` (frame_shape): HxWx3 u8
+    BGR frames, or raw camera frames, which move fewer bytes (NV12, I420: half; YUY2: two thirds) or, for BGRX, a
+    third more.  Page-locked sources (detected with cudaPointerGetAttributes) are copied
     directly; pageable ones are staged through an internal pinned ring."""
 
     def __init__(self, size, depth=2, device="cuda", pixel_format="BGR"):
@@ -256,9 +379,10 @@ class FrameUploader:
 
     @staticmethod
     def frame_shape(size, pixel_format):
-        """Shape of a host frame of size (width, height): (h, w, 3) for BGR, (3h/2, w) for NV12."""
+        """Shape of a host frame of size (width, height): (h, w, 3) for BGR, (3h/2, w) for NV12 and I420, (h, w, 2)
+        for YUY2, (h, w, 4) for BGRX."""
         w, h = size
-        return (h, w, 3) if pixel_format == "BGR" else (3 * h // 2, w)
+        return _FORMATS[pixel_format].shape(w, h)
 
     @staticmethod
     def _key(frame):
@@ -316,8 +440,7 @@ class FrameUploader:
 
     def upload_frame(self, f):
         """A host Frame of this uploader's format and size -> its device Frame."""
-        t = self.upload(f.y)
-        return nv12_frame(t) if self.pixel_format == "NV12" else Frame.bgr(t)
+        return pixel_frame(self.upload(f.y), self.pixel_format)
 
 
 class UploadSlot:
@@ -336,22 +459,25 @@ class UploadSlot:
 
 def check_capture_size(capture_size, size, pixel_format):
     """The (width, height) a tracker's frames arrive at: `size` (the tracking size) when capture_size is None, else
-    capture_size as a tuple of two positive ints (even for NV12).  Anything else raises ValueError."""
+    capture_size as a tuple of two positive ints (even where pixel_format needs it: NV12 and I420 an even width and
+    height, YUY2 an even width).  Anything else raises ValueError."""
     if capture_size is None:
         return tuple(int(v) for v in size)
     if not (isinstance(capture_size, (tuple, list)) and len(capture_size) == 2
             and all(np.isscalar(v) and int(v) == v and v > 0 for v in capture_size)):
         raise ValueError(f"capture_size must be (width, height) with positive integers, got {capture_size!r}")
     w, h = (int(v) for v in capture_size)
-    if pixel_format == "NV12" and (w % 2 or h % 2):
-        raise ValueError(f"an NV12 capture size must be even, got {w}x{h}")
+    try:
+        _check_size(pixel_format, w, h)
+    except ValueError as e:
+        raise ValueError(f"capture_size: {e}") from None
     return w, h
 
 
 class FrameResizer:
     """Device Frames of any size and format -> BGR Frames of one size (`size`, the tracking size): cv2.resize with the
-    default INTER_LINEAR of the frame (of its cv2.cvtColor decode for NV12), bit for bit, one fm_frame_resize launch on
-    the current stream into the next slot of a ring of `depth` device frames.
+    default INTER_LINEAR of the frame (of its cv2.cvtColor decode for the raw formats), bit for bit, one fm_frame_resize
+    launch on the current stream into the next slot of a ring of `depth` device frames.
 
     Slot reuse: a tracker resizes on the main stream at the start of a step, and every stage reads the resized frame
     either on the main stream or on a stream that waits on an event recorded after the resize (the detector and ReID
@@ -376,20 +502,10 @@ class FrameResizer:
 
 
 def as_frame(frame, pixel_format="BGR", size=None):
-    """A caller's frame as a Frame, nothing copied.  A Frame passes through; otherwise `frame` is in pixel_format:
-    'BGR' -- an HxWx3 uint8 cuda tensor (contiguous) or host ndarray; 'NV12' -- any form nv12_frame accepts.  size:
-    the (width, height) the frame must have; another size raises ValueError."""
-    if isinstance(frame, Frame):
-        f = frame
-    elif pixel_format == "NV12":
-        f = nv12_frame(frame)
-    elif torch.is_tensor(frame):
-        f = Frame.bgr(frame)
-    else:
-        if not (isinstance(frame, np.ndarray) and frame.dtype == np.uint8 and frame.ndim == 3 and frame.shape[2] == 3):
-            raise ValueError(f"BGR host frame: expected an HxWx3 uint8 ndarray, got {type(frame).__name__} "
-                             f"{getattr(frame, 'dtype', '')} {getattr(frame, 'shape', '')}")
-        f = Frame("BGR", frame.shape[1], frame.shape[0], frame)
+    """A caller's frame as a Frame, nothing copied.  A Frame passes through; otherwise `frame` is in pixel_format, in
+    any form pixel_frame accepts ('BGR': an HxWx3 uint8 cuda tensor (contiguous) or host ndarray).  size: the (width,
+    height) the frame must have; another size raises ValueError."""
+    f = frame if isinstance(frame, Frame) else pixel_frame(frame, pixel_format)
     if size is not None and f.size != tuple(size):
         raise ValueError(f"{f.format} frame of size {f.size}, expected {tuple(size)}")
     return f

@@ -60,7 +60,7 @@ class FeatureExtractor:
         return self.model.METRIC
 
     def extract_async(self, frame, tlbrs):
-        """frame: HxWx3 u8 host array or cuda tensor, or a Frame (an NV12 frame is read in place); tlbrs: (N,4)."""
+        """frame: HxWx3 u8 host array or cuda tensor, or a Frame (of any pixel format, read in place); tlbrs: (N,4)."""
         tlbrs = np.ascontiguousarray(tlbrs, np.float64).reshape(-1, 4)
         n = len(tlbrs)
         self.last_num_features = n

@@ -272,7 +272,8 @@ class Flow:
 
     # ------------------------------------------------------------------
     def _to_device(self, frame):
-        """The device Frame of a frame of this stage's size (BGR, or an NV12 Frame); host frames are uploaded."""
+        """The device Frame of a frame of this stage's size (BGR, or a Frame of any pixel format); host frames are
+        uploaded."""
         return device_frame(frame, self._upload, size=self.size)
 
     def _preprocess(self, frame_dev, k):

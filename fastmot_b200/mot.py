@@ -45,17 +45,24 @@ class MOT:
                  embeddings_tap=None,
                  pixel_format='BGR',
                  capture_size=None):
-        """pixel_format: 'BGR' -- every frame is HxWx3 u8 (host array or cuda tensor); 'NV12' -- every frame is NV12
-        as hardware video decoders emit it, in any form devmem.nv12_frame accepts (host (3H/2, W) array, pitched cuda
-        tensor, or a (Y, UV) pair of cuda planes).  NV12 frames are read in place by the letterbox, crop and KLT
-        kernels; tracks, detections and embeddings are those of the BGR path on cv2.cvtColor(frame,
-        cv2.COLOR_YUV2BGR_NV12).
+        """pixel_format: the layout every frame arrives in, in any form devmem.pixel_frame accepts for it:
+          'BGR'  -- HxWx3 u8 (host array or cuda tensor);
+          'NV12' -- as hardware video decoders and CSI cameras emit it (host (3H/2, W) array, pitched cuda tensor, or a
+                    (Y, UV) pair of cuda planes);
+          'I420' -- as software decoders (and PyAV / FFmpeg yuv420p) emit it (host (3H/2, W) array, tight cuda tensor,
+                    or a (Y, U, V) triple of cuda planes);
+          'YUY2' -- as USB cameras emit it (host or pitched cuda (H, W, 2));
+          'BGRX' -- as nvvidconv emits it (host or pitched cuda (H, W, 4)).
+        Raw frames are read in place by the letterbox, crop and KLT kernels; tracks, detections and embeddings are
+        those of the BGR path on cv2.cvtColor(frame, code), code = COLOR_YUV2BGR_NV12, _I420, _YUY2 or
+        COLOR_BGRA2BGR.
 
         size is the tracking size (the reference's resize_to).  capture_size: the (width, height) of the frames `step`
-        and `prefetch` receive (the reference's stream_cfg.resolution; even for NV12), when it differs from `size`.
-        Each frame is uploaded at that size and scaled to `size` on the GPU, bit for bit cv2.resize(frame, size) with
-        INTER_LINEAR (of the cv2 decode for NV12); tracks and boxes are in tracking-size coordinates, as in the
-        reference.  None, or capture_size == size, tracks the frames as they come."""
+        and `prefetch` receive (the reference's stream_cfg.resolution; even for NV12 and I420, an even width for
+        YUY2), when it differs from `size`.  Each frame is uploaded at that size and scaled to `size` on the GPU, bit
+        for bit cv2.resize(frame, size) with INTER_LINEAR (of the cv2 decode for the raw formats); tracks and boxes are
+        in tracking-size coordinates, as in the reference.  None, or capture_size == size, tracks the frames as they
+        come."""
         self.size = size
         self.pixel_format = check_pixel_format(pixel_format)
         self.capture_size = check_capture_size(capture_size, size, self.pixel_format)

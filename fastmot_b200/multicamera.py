@@ -58,11 +58,14 @@ class MultiCameraMOT:
                  draw=False,
                  detections_override=None,
                  embeddings_override=None,
-                 pixel_format='BGR',
+                 pixel_format=None,
                  capture_size=None,
-                 capture_sizes=None):
-        """sizes: one (width, height) tracking size per camera.  pixel_format ('BGR' or 'NV12', as in MOT) applies to
-        every camera of the group.  The keyword arguments are MOT's, so the reference's `mot_cfg`
+                 capture_sizes=None,
+                 pixel_formats=None):
+        """sizes: one (width, height) tracking size per camera.  pixel_formats: one pixel format per camera (any of
+        MOT's: 'BGR', 'NV12', 'I420', 'YUY2', 'BGRX'), e.g. a USB camera (YUY2), an RTSP camera (I420) and a CSI
+        camera (NV12) in one group; pixel_format: one format for every camera (MOT's keyword); give at most one of the
+        two (neither: 'BGR').  The keyword arguments are MOT's, so the reference's `mot_cfg`
         (cfg/mot.json) passes unchanged; ssd_detector_cfg, public_detector_cfg and visualizer_cfg are accepted and
         unused, since only the YOLO detector runs several cameras.  detections_override(camera, frame_id) and
         embeddings_override(camera, frame_id, detections) replace the networks' OUTPUT after both ran, as MOT's hooks
@@ -79,7 +82,20 @@ class MultiCameraMOT:
                 raise ValueError(f"every camera size must be (width, height), got {wh!r}")
             self.sizes.append(tuple(int(v) for v in wh))
         self.num_cameras = N = len(self.sizes)
-        self.pixel_format = check_pixel_format(pixel_format)
+        if pixel_format is not None and pixel_formats is not None:
+            raise ValueError("give pixel_format (every camera) or pixel_formats (one per camera), not both")
+        if pixel_formats is None:
+            pixel_formats = [pixel_format or 'BGR'] * N
+        if len(pixel_formats) != N:
+            raise ValueError(f"pixel_formats: expected {N} entries (one per camera), got {len(pixel_formats)}")
+        self.pixel_formats = []
+        for s, fmt in enumerate(pixel_formats):
+            try:
+                self.pixel_formats.append(check_pixel_format(fmt))
+            except ValueError as e:
+                raise ValueError(f"camera {s}: {e}") from None
+        # the group's one format, None for a group of several
+        self.pixel_format = self.pixel_formats[0] if len(set(self.pixel_formats)) == 1 else None
         if capture_size is not None and capture_sizes is not None:
             raise ValueError("give capture_size (every camera) or capture_sizes (one per camera), not both")
         if capture_sizes is None:
@@ -87,9 +103,9 @@ class MultiCameraMOT:
         if len(capture_sizes) != N:
             raise ValueError(f"capture_sizes: expected {N} entries (one per camera), got {len(capture_sizes)}")
         self.capture_sizes = []
-        for s, (cs, wh) in enumerate(zip(capture_sizes, self.sizes)):
+        for s, (cs, wh, fmt) in enumerate(zip(capture_sizes, self.sizes, self.pixel_formats)):
             try:
-                self.capture_sizes.append(check_capture_size(cs, wh, self.pixel_format))
+                self.capture_sizes.append(check_capture_size(cs, wh, fmt))
             except ValueError as e:
                 raise ValueError(f"camera {s}: {e}") from None
         self.detector_type = DetectorType[detector_type.upper()]
@@ -124,7 +140,8 @@ class MultiCameraMOT:
         self.trackers = [MultiTracker(wh, self.extractors[0].metric, **vars(tracker_cfg),
                                       feat_dim=self.extractors[0].feature_dim) for wh in self.sizes]
         self.frame_counts = [0] * N
-        self._uploaders = [FrameUploader(wh, depth=3, pixel_format=self.pixel_format) for wh in self.capture_sizes]
+        self._uploaders = [FrameUploader(wh, depth=3, pixel_format=fmt)
+                           for wh, fmt in zip(self.capture_sizes, self.pixel_formats)]
         self._resizers = [None if cs == wh else FrameResizer(wh) for cs, wh in zip(self.capture_sizes, self.sizes)]
         self._det_stream = torch.cuda.Stream()
         self._main_ready = torch.cuda.Event()
@@ -153,14 +170,14 @@ class MultiCameraMOT:
         self._each_frame(prefetch_frame, frames)
 
     def _each_frame(self, fn, frames):
-        """[fn(frame, camera's uploader, pixel format, camera's capture size) or None] over the cameras' frames (None:
-        no frame); a frame of the wrong size or form raises ValueError naming its camera."""
+        """[fn(frame, camera's uploader, camera's pixel format, camera's capture size) or None] over the cameras' frames
+        (None: no frame); a frame of the wrong size or form raises ValueError naming its camera."""
         if len(frames) != self.num_cameras:
             raise ValueError(f"expected {self.num_cameras} frames, got {len(frames)}")
         out = []
-        for s, (f, up, wh) in enumerate(zip(frames, self._uploaders, self.capture_sizes)):
+        for s, (f, up, fmt, wh) in enumerate(zip(frames, self._uploaders, self.pixel_formats, self.capture_sizes)):
             try:
-                out.append(None if f is None else fn(f, up, self.pixel_format, wh))
+                out.append(None if f is None else fn(f, up, fmt, wh))
             except ValueError as e:
                 raise ValueError(f"camera {s}: {e}") from None
         return out
@@ -178,8 +195,8 @@ class MultiCameraMOT:
         return dict(zip(cams, dets))
 
     def step(self, frames):
-        """One step of the group: frames[s] is camera s's next frame in the group's pixel format (HxWx3 u8 host array
-        or cuda tensor; NV12 in any form MOT takes), or None when camera s has no frame on this step."""
+        """One step of the group: frames[s] is camera s's next frame in its pixel format, in any form MOT takes for
+        that format (HxWx3 u8 host array or cuda tensor for BGR), or None when camera s has no frame on this step."""
         frames_dev = self._each_frame(device_frame, frames)
         # scaled cameras: resized on the main stream, before _main_ready is recorded (devmem.FrameResizer)
         frames_dev = [f if f is None or r is None else r.resize(f) for f, r in zip(frames_dev, self._resizers)]

@@ -27,8 +27,8 @@ class MultiStreamMOT(MultiCameraMOT):
                  embeddings_override=None,
                  pixel_format='BGR',
                  capture_size=None):
-        """size: (width, height) shared by every stream; pixel_format ('BGR' or 'NV12', as in MOT) applies to every
-        stream.  The keyword arguments are MOT's, so the reference's
+        """size: (width, height) shared by every stream; pixel_format (any of MOT's: 'BGR', 'NV12', 'I420', 'YUY2',
+        'BGRX') applies to every stream.  The keyword arguments are MOT's, so the reference's
         `mot_cfg` (cfg/mot.json) passes unchanged; ssd_detector_cfg, public_detector_cfg and visualizer_cfg are
         accepted and unused, since only the YOLO detector runs several streams.  detections_override(stream,
         frame_id) and embeddings_override(stream, frame_id, detections) replace the networks' OUTPUT after both ran,
@@ -55,8 +55,8 @@ class MultiStreamMOT(MultiCameraMOT):
         return self.frame_counts[0]
 
     def step(self, frames):
-        """One step of every stream: frames[s] is stream s's next frame (HxWx3 u8 host array or cuda tensor; NV12 in
-        any form MOT takes when pixel_format is 'NV12')."""
+        """One step of every stream: frames[s] is stream s's next frame, in any form MOT takes for the pixel format
+        (HxWx3 u8 host array or cuda tensor for BGR)."""
         if any(f is None for f in frames):
             raise ValueError("every stream delivers a frame on every step; cameras that skip steps need "
                              "MultiCameraMOT")

@@ -163,25 +163,38 @@ typedef struct FmYoloHead {
     float scale_x_y;
 } FmYoloHead;
 
-/* Pixel formats of the frames the letterbox, crop and KLT gray kernels read.  NV12 (what hardware video decoders
- * emit): a Y plane of h rows and a UV plane of h / 2 rows, both w bytes wide (U, V interleaved at half resolution),
- * each with its own row pitch in bytes, w and h even.  Every entry gives on an NV12 frame bit for bit what it gives on
- * the BGR frame cv2.cvtColor(frame, cv2.COLOR_YUV2BGR_NV12) (OpenCV 4.13: BT.601 limited range, 20-bit fixed point,
+/* Pixel formats of the frames the letterbox, crop, KLT gray and frame-resize kernels read, read in place:
+ *   NV12 (hardware video decoders, CSI cameras): a Y plane of h rows and a UV plane of h / 2 rows, both w bytes wide
+ *        (U, V interleaved at half resolution);
+ *   I420 (software decoders, PyAV / FFmpeg yuv420p): a Y plane of h rows, then a U and a V plane of h / 2 rows of
+ *        w / 2 bytes;
+ *   YUY2 (USB / V4L2 cameras): one packed plane of h rows of 2w bytes, Y0 U Y1 V per pixel pair;
+ *   BGRX (nvvidconv's BGRx): one packed plane of h rows of 4w bytes, B G R x per pixel (x is not read).
+ * Every entry gives on such a frame bit for bit what it gives on the BGR frame cv2.cvtColor(frame, code), code =
+ * COLOR_YUV2BGR_NV12, _I420, _YUY2 or COLOR_BGRA2BGR (OpenCV 4.13: BT.601 limited range, 20-bit fixed point,
  * nearest-neighbour chroma); the pixels are converted inline, no BGR frame is written. */
 #define FM_PIX_BGR 0
 #define FM_PIX_NV12 1
+#define FM_PIX_I420 2
+#define FM_PIX_YUY2 3
+#define FM_PIX_BGRX 4
 
-/* One camera frame in device memory, as every entry that reads camera pixels takes it.
- *   FM_PIX_BGR : y is the tight u8 HWC frame (w * 3 bytes per row); uv, pitch and uv_pitch are ignored.
- *   FM_PIX_NV12: y and uv are the two planes, pitch and uv_pitch their row pitches in bytes (0 = w, else >= w).
- * The one-frame entries take a host pointer to it and reject a NULL y, an empty frame, an unknown format and an NV12
- * frame that breaks the rules above. */
+/* One camera frame in device memory, as every entry that reads camera pixels takes it.  Row pitches are in bytes.
+ *   FM_PIX_BGR : y is the tight u8 HWC frame (w * 3 bytes per row); uv, v, pitch and uv_pitch are ignored.
+ *   FM_PIX_NV12: y and uv are the two planes, pitch and uv_pitch their row pitches (0 = w, else >= w); w, h even.
+ *   FM_PIX_I420: y is the Y plane with row pitch `pitch` (0 = w, else >= w), uv the U plane and v the V plane, which
+ *                share the row pitch uv_pitch (0 = w / 2, else >= w / 2); w, h even.
+ *   FM_PIX_YUY2: y is the packed plane, pitch its row pitch (0 = 2w, else >= 2w); w even; uv, v, uv_pitch ignored.
+ *   FM_PIX_BGRX: y is the packed plane, pitch its row pitch (0 = 4w, else >= 4w); uv, v, uv_pitch ignored.
+ * The one-frame entries take a host pointer to it and reject a NULL y, an empty frame, an unknown format and a frame
+ * that breaks the rules above.  v was appended last, so the other fields keep their offsets. */
 typedef struct FmFrame {
     const unsigned char* y;
     const unsigned char* uv;
     int w, h;
     int pitch, uv_pitch;
     int format;
+    const unsigned char* v;
 } FmFrame;
 
 /* One frame of a batch whose frames may differ in size: the device frame, its letterbox ROI in the network input, and
@@ -196,7 +209,7 @@ typedef struct FmFrameGeom {
 /* YOLODetector._preprocess + _create_letterbox (fastmot/detector.py:289-320): bilinear resize of the frame into the
  * ROI [roi_x, roi_y, roi_w, roi_h] of a dst_w x dst_h network input (half-pixel centres, edge replicate, rounded to u8
  * like the reference's CuPy zoom), BGR->RGB, x/255; everything outside the ROI = 0.5.  An NV12 frame's four bilinear
- * taps are each converted to BGR with their own chroma sample before they are interpolated.
+ * taps (of any YUV format) are each converted to BGR with their own chroma sample before they are interpolated.
  * layout 0: fp32 planar CHW (the reference's TensorRT input); layout 1: fp16 NHWC, C padded to 8 (16 bytes per pixel). */
 int fm_letterbox_preproc(const FmFrame* frame, int dst_w, int dst_h, int roi_x, int roi_y, int roi_w, int roi_h,
                          int layout, void* out, void* stream);
@@ -207,7 +220,7 @@ int fm_letterbox_preproc_geom(const FmFrameGeom* geom, int batch, int dst_w, int
 
 /* FeatureExtractor.extract_async preprocessing (fastmot/feature_extractor.py:48-60, 84-98; rect.py:92-97) for all
  * crops in one launch: integer-truncated clamp crop, OpenCV INTER_LINEAR 8-bit fixed-point resize to
- * out_w x out_h, BGR->RGB, (x/255 - mean)/std (an NV12 frame's taps are converted to BGR before they are
+ * out_w x out_h, BGR->RGB, (x/255 - mean)/std (a YUV frame's taps are converted to BGR before they are
  * interpolated).  n = min(*n_dev, n_max) if n_dev != NULL else n_max.
  * layout as above; output is [n][3][out_h][out_w] f32 or [n][out_h][out_w][8] f16; layout 2: fp16
  * [n][out_h + 8][out_w + 8][4] with the crop at (+4, +4) inside a border the CALLER zeroed once (the zero padding of
@@ -222,8 +235,8 @@ int fm_roi_resize_norm_geom(const FmFrameGeom* geom, const int* frame_idx, const
                             int out_h, int layout, void* out, void* stream);
 
 /* cv2.resize(bgr(src), (dw, dh)) with the default INTER_LINEAR into a tight dh x dw x 3 u8 BGR frame.  bgr(src) is
- * src itself for FM_PIX_BGR, cv2.cvtColor(src, COLOR_YUV2BGR_NV12) for FM_PIX_NV12 (read in place, as the letterbox
- * / crop / gray kernels read it).  dst must not overlap src.  Bit-identical to OpenCV 4.13: an exact 2x downscale in
+ * src itself for FM_PIX_BGR, cv2.cvtColor(src, code) for the other formats, code as listed at FM_PIX_BGR (read in
+ * place, as the letterbox / crop / gray kernels read it).  dst must not overlap src.  Bit-identical to OpenCV 4.13: an exact 2x downscale in
  * both axes is the 2x2 rounded mean, every other size pair the 11-bit fixed-point generic path.  Any size pair is
  * accepted (dh <= 65535); capture frames tracked at another size go through it (a camera's stream_cfg.resolution ->
  * resize_to). */
