@@ -342,10 +342,14 @@ __device__ void affine_partial_from2(const float* f0, const float* f1, const flo
     M[3] = S1; M[4] = S0; M[5] = S3;
 }
 
+// Affine2DEstimatorCallback::computeError: the model rounded to float and the residual formed in float, each operation
+// rounded on its own (no FMA contraction), so a point within rounding of the threshold falls on OpenCV's side of it
 __device__ __forceinline__ bool affine_inlier(const double* F, const float* f, const float* t, double thr2) {
-    const double a = F[0] * f[0] + F[1] * f[1] + F[2] - t[0];
-    const double b = F[3] * f[0] + F[4] * f[1] + F[5] - t[1];
-    const float e = (float)(a * a + b * b);
+    const float a = __fsub_rn(__fadd_rn(__fadd_rn(__fmul_rn((float)F[0], f[0]), __fmul_rn((float)F[1], f[1])),
+                                        (float)F[2]), t[0]);
+    const float b = __fsub_rn(__fadd_rn(__fadd_rn(__fmul_rn((float)F[3], f[0]), __fmul_rn((float)F[4], f[1])),
+                                        (float)F[5]), t[1]);
+    const float e = __fadd_rn(__fmul_rn(a, a), __fmul_rn(b, b));
     return (double)e <= thr2;
 }
 
@@ -433,7 +437,7 @@ __global__ void __launch_bounds__(128) affine_partial_kernel(
     // ---- RANSAC ----
     const double thr2 = thresh * thresh;
     __shared__ CvRng s_rng;
-    if (tid == 0) { s_rng.state = 0xffffffffffffffffULL; s_niters = max_iters; s_maxgood = 0; s_iter = 0; s_done = 0; }
+    if (tid == 0) { s_rng.state = 0xffffffffffffffffULL; s_niters = max(max_iters, 1); s_maxgood = 0; s_iter = 0; s_done = 0; }
     __syncthreads();
     while (true) {
         if (tid == 0) {
@@ -698,11 +702,14 @@ __device__ bool homography_from4(const float* M /* src 4x2 */, const float* mm /
     return true;
 }
 
+// HomographyEstimatorCallback::computeError in float, each operation rounded on its own (no FMA contraction)
 __device__ __forceinline__ bool homography_inlier(const float* Hf, const float* M, const float* m, double thr2) {
-    const float ww = 1.f / (Hf[6] * M[0] + Hf[7] * M[1] + 1.f);
-    const float dx = (Hf[0] * M[0] + Hf[1] * M[1] + Hf[2]) * ww - m[0];
-    const float dy = (Hf[3] * M[0] + Hf[4] * M[1] + Hf[5]) * ww - m[1];
-    const float e = dx * dx + dy * dy;
+    const float ww = __fdiv_rn(1.f, __fadd_rn(__fadd_rn(__fmul_rn(Hf[6], M[0]), __fmul_rn(Hf[7], M[1])), 1.f));
+    const float dx = __fsub_rn(__fmul_rn(__fadd_rn(__fadd_rn(__fmul_rn(Hf[0], M[0]), __fmul_rn(Hf[1], M[1])), Hf[2]), ww),
+                               m[0]);
+    const float dy = __fsub_rn(__fmul_rn(__fadd_rn(__fadd_rn(__fmul_rn(Hf[3], M[0]), __fmul_rn(Hf[4], M[1])), Hf[5]), ww),
+                               m[1]);
+    const float e = __fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy));
     return (double)e <= thr2;
 }
 
@@ -792,7 +799,8 @@ __global__ void __launch_bounds__(256) homography_kernel(const float* __restrict
         return;
     }
     HOM_STAMP(1);
-    if (tid == 0) { s_rng.state = 0xffffffffffffffffULL; s_niters = max_iters; s_maxgood = 0; s_iter = 0; s_done = 0; }
+    // niters = MAX(maxIters, 1): one hypothesis is drawn even when maxIters is 0
+    if (tid == 0) { s_rng.state = 0xffffffffffffffffULL; s_niters = max(max_iters, 1); s_maxgood = 0; s_iter = 0; s_done = 0; }
     __syncthreads();
     while (true) {
         if (tid == 0) {
@@ -976,15 +984,39 @@ __global__ void __launch_bounds__(256) homography_kernel(const float* __restrict
     }
     __syncthreads();
     HOM_STAMP(6);
+    // ---- the mask findHomography returns: every match whose error under the refined model is within the threshold ----
+    if (tid < 8) s_bestf[tid] = (float)s_x[tid];
+    if (tid == 0) s_ninl = 0;
+    __syncthreads();
+    for (int base = 0; base < n; base += blockDim.x) {
+        const int i = base + tid;
+        bool in = false;
+        if (i < n) { const int p = good_idx[i]; in = homography_inlier(s_bestf, all_prev + 2 * p, all_cur + 2 * p, thr2); }
+        const unsigned bal = __ballot_sync(0xffffffffu, in);
+        if (lane == 0) s_warpcnt[wid] = __popc(bal);
+        __syncthreads();
+        int off = s_ninl;
+        for (int w = 0; w < wid; ++w) off += s_warpcnt[w];
+        off += __popc(bal & ((1u << lane) - 1));
+        if (in) inl_idx[off] = good_idx[i];
+        __syncthreads();
+        if (tid == 0) {
+            int t = 0;
+            for (int w = 0; w < 8; ++w) t += s_warpcnt[w];
+            s_ninl += t;
+        }
+        __syncthreads();
+    }
+    const int n_fin = s_ninl;
     if (g_hom_dbg && tid == 0) g_hom_dbg[10] = (unsigned long long)n_in;
     if (tid == 0) {
         for (int i = 0; i < 8; ++i) H_out[i] = s_x[i];
         H_out[8] = 1.0;
-        const bool ok = n_in >= inlier_thresh;
+        const bool ok = n_fin >= inlier_thresh;
         *h_ok = ok ? 1 : 0;
-        *bg_kp_count = ok ? min(n_in, max_bg) : 0;
+        *bg_kp_count = ok ? min(n_fin, max_bg) : 0;
     }
-    for (int i = tid; i < min(n_in, max_bg); i += blockDim.x) {
+    for (int i = tid; i < min(n_fin, max_bg); i += blockDim.x) {
         const int p = inl_idx[i];
         bg_kp[2 * i] = all_cur[2 * p]; bg_kp[2 * i + 1] = all_cur[2 * p + 1];
         bg_kp_prev[2 * i] = all_prev[2 * p]; bg_kp_prev[2 * i + 1] = all_prev[2 * p + 1];
