@@ -382,6 +382,132 @@ def build_yolo_engine(model, weights=None, use_tc=True, use_graph=True, head_obj
     return YoloEngine(layers, model.INPUT_SHAPE[1:], weights, use_tc=use_tc, use_graph=use_graph, batch=batch)
 
 
+class LaunchGroup:
+    """One launch of an OSNet engine: its trace `kind`, the range of `ops` it implements, the (c, h, w) `shape` its
+    last op writes, and the kind-specific details its emitter needs in `info`."""
+    __slots__ = ("kind", "ops", "shape", "info")
+
+    def __init__(self, kind, ops, shape, info):
+        self.kind, self.ops, self.shape, self.info = kind, ops, shape, info
+
+
+def _reads(op):
+    """The buffer names an OSNet op reads."""
+    kind = op[0]
+    if kind == 'conv':
+        return [op[8]]
+    if kind == 'dw':
+        return [op[4]]
+    if kind in ('maxpool3s2', 'avgpool2', 'gap'):
+        return [op[1]]
+    if kind == 'gate':
+        return [op[3], op[4]]
+    if kind == 'gate4':
+        return list(op[3])
+    if kind == 'add_relu':
+        return [op[1], op[2]]
+    if kind == 'fc':
+        return [op[4]]
+    return []
+
+
+def _match_osblock(ops, k):
+    """ops[k] = '<blk>.conv1'; returns (tail buffer names of the four streams, index of the gate4 op) when the next
+    twenty ops are the Lite-3x3 chains a.0, b.0, b.1, c.0 .. d.3 feeding that gate, else None."""
+    if k + 21 >= len(ops):
+        return None
+    x1 = ops[k][9]
+    mid = ops[k][3]
+    tails = []
+    i = k + 1
+    for s_ in range(4):
+        prev = x1
+        for j in range(s_ + 1):
+            pw, dw = ops[i], ops[i + 1]
+            if pw[0] != 'conv' or dw[0] != 'dw' or pw[2] != mid or pw[3] != mid or pw[4] != 1 or pw[7] != 'linear' \
+                    or pw[8] != prev or dw[4] != pw[9] or dw[2] != mid or dw[3] != 'relu':
+                return None
+            prev = dw[5]
+            i += 2
+        tails.append(prev)
+    g = ops[i]
+    if g[0] != 'gate4' or tuple(g[3]) != tuple(tails):
+        return None
+    return tails, i
+
+
+def _match_merge(ops, k):
+    """ops[k] = gate4 of an OSBlock; returns (downsample conv or None, conv3, add_relu, index of add_relu) when
+    the ops that follow are [downsample 1x1] conv3 1x1 (linear, reads the gate output) and add_relu."""
+    acc = ops[k][4]
+    i = k + 1
+    ds = None
+    if i < len(ops) and ops[i][0] == 'conv' and ops[i][8] != acc:      # a conv beside conv3: the downsample branch
+        ds = ops[i]
+        i += 1
+    if i + 1 >= len(ops):
+        return None
+    c3, add = ops[i], ops[i + 1]
+    if c3[0] != 'conv' or c3[4] != 1 or c3[7] != 'linear' or c3[8] != acc or add[0] != 'add_relu':
+        return None
+    if c3[9] not in (add[1], add[2]):
+        return None
+    other = add[2] if add[1] == c3[9] else add[1]
+    if ds is not None and (ds[4] != 1 or ds[7] != 'linear' or ds[9] != other or ds[2] % 64):
+        return None
+    return ds, c3, add, i + 1
+
+
+def plan_osnet(ops, input_hw, fuse_osb, lib):
+    """The launches an OSNet op list becomes, in order: LaunchGroups whose op ranges cover every op exactly once.
+    Every fusion decision of the engine is taken here, from the ops and their shapes alone (no device):
+      'stem'          the 7x7/2 conv + 3x3/2 max-pool of a 256x128 input in one launch (fm_osnet_stem);
+      'S'             an OSBlock's conv1 and its four Lite-3x3 streams (fm_osb_streams), which also writes the strip
+                      sums of the tails; info: the tail names and the strip count;
+      'G'             the gate4 over S's tails, [downsample,] conv3 and the residual add + ReLU (fm_osb_merge); info:
+                      the downsample (or None), conv3 and add_relu ops and the output channels per CTA;
+      'gate4_pooled'  a gate4 over S's tails that the merge kernel cannot take, reading S's strip sums;
+      'conv+add'      a linear conv whose output feeds add_relu next: the add and ReLU run in the conv epilogue;
+      and one group per remaining op, of that op's kind.
+    `fuse_osb` False keeps one launch per op apart from conv+add.  `lib` answers which geometries the fused OSBlock
+    kernels support (fm_osb_streams_strips, fm_osb_merge_ncta: host-only functions)."""
+    shapes = osnet.infer_shapes(ops, *input_hw)
+    groups, strips_of = [], {}      # strips_of: first tail name of an S group -> its strip count
+
+    def group(kind, k, end, **info):
+        groups.append(LaunchGroup(kind, tuple(range(k, end)), shapes[end - 1], info))
+        return end
+
+    k = 0
+    if fuse_osb and tuple(input_hw) == (256, 128) and len(ops) > 1 and ops[0][0] == 'conv' \
+            and ops[0][2:8] == (3, 64, 7, 2, 3, 'relu') and ops[1][0] == 'maxpool3s2' and ops[1][1] == ops[0][9]:
+        k = group('stem', 0, 2)
+    while k < len(ops):
+        op = ops[k]
+        nxt = ops[k + 1] if k + 1 < len(ops) else ('end',)
+        if op[0] == 'conv':
+            # kernel S computes conv1 as a 1x1, stride-1, unpadded conv: at its input's shape
+            blk = _match_osblock(ops, k) if fuse_osb and op[4:8] == (1, 1, 0, 'relu') and op[2] % 64 == 0 else None
+            strips = lib.fm_osb_streams_strips(shapes[k][1], shapes[k][2], op[3]) if blk else 0
+            if strips > 0:
+                strips_of[blk[0][0]] = strips
+                k = group('S', k, blk[1], tails=blk[0], strips=strips)
+            elif nxt[0] == 'add_relu' and nxt[1] == op[9] and nxt[2] != op[9] and op[7] == 'linear':
+                k = group('conv+add', k, k + 2)
+            else:
+                k = group('conv', k, k + 1)
+        elif op[0] == 'gate4' and op[3][0] in strips_of:
+            m = _match_merge(ops, k)
+            ncta = lib.fm_osb_merge_ncta(op[2], m[1][3]) if m else 0
+            if ncta > 0:
+                k = group('G', k, m[3] + 1, ds=m[0], c3=m[1], add=m[2], ncta=ncta)
+            else:
+                k = group('gate4_pooled', k, k + 1)
+        else:
+            k = group(op[0], k, k + 1)
+    return groups
+
+
 class OSNetEngine(_Net):
     """OSNet executor for up to `max_batch` crops per call: forward(x [n,256,128,8] fp16, n) -> [n, 512] f32
     L2-normalised embeddings (feature_extractor.py:62-74)."""
@@ -406,10 +532,8 @@ class OSNetEngine(_Net):
         # FM_OSB_FUSED=0 falls back to one launch per layer (r01 path); default: fused stem (fm_osnet_stem), one
         # fm_osb_streams + fm_osb_merge pair per OSBlock (csrc/osnet_fused.cu, csrc/osnet_stem.cu)
         self.fuse_osb = os.environ.get("FM_OSB_FUSED", "1") != "0" and use_tc
-        first, second = self.ops[0], self.ops[1]
-        self.fuse_stem = (self.fuse_osb and (H, W) == (256, 128) and first[0] == 'conv'
-                          and first[2:8] == (3, 64, 7, 2, 3, 'relu') and second[0] == 'maxpool3s2'
-                          and second[1] == first[9])
+        plan = plan_osnet(self.ops, (H, W), self.fuse_osb, self._lib)
+        self.fuse_stem = plan[0].kind == 'stem'
         # network input: NHWC8 (layout 1 of fm_roi_resize_norm) or, for the fused stem, NHWC4 inside a zero border
         self.inp_layout = 2 if self.fuse_stem else 1
         if self.fuse_stem:
@@ -417,358 +541,258 @@ class OSNetEngine(_Net):
         else:
             self.inp = torch.zeros(B, H, W, IN_C_PAD, dtype=torch.float16, device=dev)
         self.out = torch.zeros(B, feature_dim, dtype=torch.float32, device=dev)
-        self.n_dev = None
-        # last use of every symbolic buffer -> simple size-keyed recycling
-        last = {}
-        for k, op in enumerate(self.ops):
-            for name in self._reads(op):
-                last[name] = k
-        pool = {}
-        live = {'input': (self.inp, IN_C_PAD, H, W)}
-        params = {}
-
-        self._bufs = []     # every activation buffer must outlive the recorded launches (raw pointers!)
-
-        def alloc(numel, dtype=torch.float16):
-            key = (numel, dtype)
-            if pool.get(key):
-                return pool[key].pop()
-            t = torch.zeros(numel, dtype=dtype, device=dev)
-            self._bufs.append(t)
-            return t
-
-        def release(name):
-            t = live.pop(name, None)
-            if t is not None and name not in ('input',):
-                pool.setdefault((t[0].numel(), t[0].dtype), []).append(t[0])
-
-        def dparam(name):
-            if name not in params:
-                params[name] = tuple(torch.as_tensor(a).to(dev) for a in self.weights[name])
-            return params[name]
-
-        # self.trace[i] describes self.launches[i] (TraceEntry): which ops it implements, the views it reads and writes
-        self.trace = []
-        views = {'input': View('input', self.inp, 'nhwc4b', 4, H, W) if self.fuse_stem
-                 else View('input', self.inp, 'nhwc', IN_C_PAD, H, W)}
-
-        def nhwc(name):
-            """The NHWC view of a live buffer, recorded under its name."""
-            t_, c_, h_, w_ = live[name]
-            views[name] = View(name, t_, 'nhwc', c_, h_, w_)
-            return views[name]
-
-        def trace(kind, ks, ins, outs):
-            self.trace.append(TraceEntry(kind, ks, [views[s_] for s_ in ins], outs))
-
         self.pooled = torch.zeros(4 * B, 512, dtype=torch.float32, device=dev)
         self.gate_tmp = torch.zeros(4 * B, 512, dtype=torch.float32, device=dev)
-        self._params = params
-        fused_add = {}
+        self._params = {}
+        self._bufs = []     # every activation buffer must outlive the recorded launches (raw pointers!)
+        self._free = {}     # (numel, dtype) -> released activation buffers, reused by the next _alloc of that size
+        # name -> (tensor, channels, h, w) of the buffers a later launch still reads
+        self._live = {'input': (self.inp, IN_C_PAD, H, W)}
+        # name -> the View its last writer recorded; self.trace[i] describes self.launches[i] through these views
+        self._views = {'input': View('input', self.inp, 'nhwc4b', 4, H, W) if self.fuse_stem
+                       else View('input', self.inp, 'nhwc', IN_C_PAD, H, W)}
+        self.trace = []
         self.n_osb = 0
-        skip_until = -1
-        pooled_by_tail = {}
-        for k, op in enumerate(self.ops):
-            kind = op[0]
-            if k <= skip_until:
-                continue
-            if k == 0 and self.fuse_stem:
-                from .packing import pack_b_sw64
-                w7, b7 = self.weights[op[1]]                        # [64][7][7][3]
-                wk = np.zeros((64, 7, 8, 4), np.float32)
-                wk[:, :, 1:8, :3] = w7
-                img = torch.as_tensor(pack_b_sw64(wk.reshape(64, 224))).to(dev)
-                b_d = torch.as_tensor(np.ascontiguousarray(b7, np.float32)).to(dev)
-                y = alloc(B * 64 * 32 * 64)
-                self._keep += [img, b_d]
-                self._add('fm_osnet_stem', ptr(self.inp), B, ptr(img), ptr(b_d), ptr(y))
-                self.n_tc += 1
-                self.layer_bytes += 2 * (B * (H + 8) * (W + 8) * 4 + B * 64 * 32 * 64)
-                live[self.ops[1][2]] = (y, 64, 64, 32)
-                trace('stem', (0, 1), ['input'], [nhwc(self.ops[1][2])])
-                skip_until = 1
-                continue
-            if kind == 'conv' and self.fuse_osb and op[4] == 1 and op[7] == 'relu':     # OSBlock candidate (structural)
-                blk = self._match_osblock(k)
-                x, xc, h, w = live[op[8]]
-                if blk is not None and xc == op[2] and xc % 64 == 0 and \
-                        self._lib.fm_osb_streams_strips(h, w, op[3]) > 0:
-                    tails_names, gate_k = blk
-                    mid = op[3]
-                    strips = self._lib.fm_osb_streams_strips(h, w, mid)
-                    from .packing import pack_b_sw128
-                    w1, b1 = self.weights[op[1]]
-                    w1_img = torch.as_tensor(pack_b_sw128(w1.reshape(mid, xc))).to(dev)
-                    b1_d = torch.as_tensor(np.ascontiguousarray(b1, np.float32)).to(dev)
-                    pw_imgs, dw_blobs = [], []
-                    for i in range(10):
-                        pw_op, dw_op = self.ops[k + 1 + 2 * i], self.ops[k + 2 + 2 * i]
-                        wp, bp = self.weights[pw_op[1]]
-                        wd, bd = self.weights[dw_op[1]]
-                        pw_imgs.append(pack_b_sw128(wp.reshape(mid, mid)))
-                        dw_blobs.append(np.concatenate([np.ascontiguousarray(wd, np.float32).astype(np.float16)
-                                                        .reshape(-1).view(np.uint8),
-                                                        np.ascontiguousarray(bp, np.float32).view(np.uint8),
-                                                        np.ascontiguousarray(bd, np.float32).view(np.uint8)]))
-                    pw_d = torch.as_tensor(np.concatenate(pw_imgs)).to(dev)
-                    dw_d = torch.as_tensor(np.concatenate(dw_blobs)).to(dev)
-                    tails = [alloc(B * h * w * mid) for _ in range(4)]
-                    gap = torch.zeros(B * strips * 4 * mid, dtype=torch.float32, device=dev)
-                    d = _lib.FmOsbStreams()
-                    d.x, d.n, d.h, d.w, d.cin, d.mid = x.data_ptr(), B, h, w, xc, mid
-                    d.w1, d.b1, d.pw, d.dw = w1_img.data_ptr(), b1_d.data_ptr(), pw_d.data_ptr(), dw_d.data_ptr()
-                    for i in range(4):
-                        d.tails[i] = tails[i].data_ptr()
-                    d.gap_part = gap.data_ptr()
-                    self._keep += [d, w1_img, b1_d, pw_d, dw_d, gap]
-                    self._add('fm_osb_streams', C.byref(d))
-                    self.n_tc += 1
-                    self.n_osb += 1
-                    self.layer_bytes += 2 * (B * h * w * (xc + 4 * mid))
-                    for i, tn in enumerate(tails_names):
-                        live[tn] = (tails[i], mid, h, w)
-                        views[tn] = View(tn, tails[i], 'planar8', mid, h, w)
-                    pooled_by_tail[tails_names[0]] = (gap, strips)
-                    gname = tails_names[0] + '.gap'
-                    views[gname] = View(gname, gap, 'gap_part', mid, h, w, strips=strips)
-                    trace('S', range(k, gate_k), [op[8]], [views[tn] for tn in tails_names] + [views[gname]])
-                    # the block input may die here (no identity / downsample use): same bookkeeping as below
-                    for name in self._reads(op):
-                        if last.get(name) == k:
-                            release(name)
-                    skip_until = gate_k - 1
-                    continue
-            if kind == 'conv':
-                _, name, cin, cout, ks, stride, pad, act, src, dst = op
-                x, xc, h, w = live[src]
-                ho, wo = (h + 2 * pad - ks) // stride + 1, (w + 2 * pad - ks) // stride + 1
-                wt, bs = self.weights[name]
-                if xc != cin:  # stem: physical 4 channels
-                    wt = np.concatenate([wt, np.zeros(wt.shape[:3] + (xc - cin,), np.float32)], -1)
-                wd = torch.as_tensor(np.ascontiguousarray(wt)).to(dev).half().contiguous()
-                bd = torch.as_tensor(bs).to(dev).float().contiguous()
-                params[name] = (wd, bd)
-                y = alloc(B * ho * wo * cout)
-                nxt = self.ops[k + 1] if k + 1 < len(self.ops) else None
-                if nxt is not None and nxt[0] == 'add_relu' and nxt[1] == dst and act == 'linear' and nxt[2] in live:
-                    # relu(conv3(x) + identity): residual + activation in the conv epilogue, no extra pass
-                    d = _conv_desc(B, h, w, xc, xc, 0, ho, wo, cout, cout, 0, ks, stride, pad,
-                                   _ACT['relu'] | ACT_AFTER_RESIDUAL)
-                    d.res_stride, d.res_offset = cout, 0
-                    self._conv(d, x, wd, bd, y, residual=live[nxt[2]][0])
-                    fused_add[k + 1] = nxt[2]
-                    new = (nxt[3], (y, cout, ho, wo))
-                    trace('conv+add', (k, k + 1), [src, nxt[2]], [View(new[0], new[1][0], 'nhwc', *new[1][1:])])
-                else:
-                    d = _conv_desc(B, h, w, xc, xc, 0, ho, wo, cout, cout, 0, ks, stride, pad, _ACT[act])
-                    self._conv(d, x, wd, bd, y)
-                    new = (dst, (y, cout, ho, wo))
-                    trace('conv', (k,), [src], [View(new[0], new[1][0], 'nhwc', *new[1][1:])])
-            elif kind == 'dw':
-                _, name, c, act, src, dst = op
-                x, xc, h, w = live[src]
-                wd, bd = dparam(name)
-                wd = wd.half().contiguous()
-                params[name] = (wd, bd)
-                y = alloc(B * h * w * c)
-                self._add('fm_dwconv3', ptr(x), ptr(wd), ptr(bd), ptr(y), B, h, w, c, _ACT[act])
-                self.layer_bytes += 2 * (2 * B * h * w * c + 9 * c)
-                new = (dst, (y, c, h, w))
-                trace(kind, (k,), [src], [View(new[0], new[1][0], 'nhwc', *new[1][1:])])
-            elif kind == 'maxpool3s2':
-                x, xc, h, w = live[op[1]]
-                ho, wo = (h + 2 - 3) // 2 + 1, (w + 2 - 3) // 2 + 1
-                y = alloc(B * ho * wo * xc)
-                self._add('fm_maxpool_pad', ptr(x), ptr(y), B, h, w, xc, 3, 2, 1)
-                new = (op[2], (y, xc, ho, wo))
-                trace(kind, (k,), [op[1]], [View(new[0], new[1][0], 'nhwc', *new[1][1:])])
-            elif kind == 'avgpool2':
-                x, xc, h, w = live[op[1]]
-                y = alloc(B * (h // 2) * (w // 2) * xc)
-                self._add('fm_avgpool2', ptr(x), ptr(y), B, h, w, xc)
-                new = (op[2], (y, xc, h // 2, w // 2))
-                trace(kind, (k,), [op[1]], [View(new[0], new[1][0], 'nhwc', *new[1][1:])])
-            elif kind == 'gate':
-                _, name, c, src, acc, accumulate = op
-                x, xc, h, w = live[src]
-                w1, b1, w2, b2 = dparam(name)
-                if acc not in live:
-                    live[acc] = (alloc(B * h * w * c), c, h, w)
-                a = live[acc][0]
-                self._add('fm_channel_gate', ptr(x), ptr(self.pooled), ptr(self.gate_tmp), ptr(w1), ptr(b1), ptr(w2),
-                          ptr(b2), ptr(a), B, h * w, c, w1.shape[0], accumulate)
-                trace(kind, (k,), [src, acc] if accumulate else [src], [nhwc(acc)])
-                new = None
-            elif kind == 'gate4' and op[3][0] in pooled_by_tail and self._match_merge(k) is not None and \
-                    self._lib.fm_osb_merge_ncta(op[2], self._match_merge(k)[1][3]) > 0:
-                # gate + conv3 (+ downsample) + residual + ReLU in one launch (kernel G)
-                _, name, c, srcs, acc = op
-                ds_op, c3_op, add_op, last_k = self._match_merge(k)
-                from .packing import pack_b_sw128
-                xs = [live[s_][0] for s_ in srcs]
-                _, _, h, w = live[srcs[0]]
-                gap, strips = pooled_by_tail[srcs[0]]
-                gw1, gb1, gw2, gb2 = dparam(name)
-                cout = c3_op[3]
-                ncta = self._lib.fm_osb_merge_ncta(c, cout)
-                w3, b3 = self.weights[c3_op[1]]
-                wcat = w3.reshape(cout, c)
-                bias = np.asarray(b3, np.float32).copy()
-                ident_name = add_op[2] if add_op[1] == c3_op[9] else add_op[1]
-                d = _lib.FmOsbMerge()
-                if ds_op is not None:
-                    wdn, bdn = self.weights[ds_op[1]]
-                    cin = ds_op[2]
-                    wcat = np.concatenate([wdn.reshape(cout, cin), wcat], 1)
-                    bias += np.asarray(bdn, np.float32)
-                    xin = live[ds_op[8]]
-                    d.x, d.res, d.cin = xin[0].data_ptr(), None, cin
-                else:
-                    d.x, d.res, d.cin = None, live[ident_name][0].data_ptr(), cout
-                img = np.concatenate([pack_b_sw128(wcat[r:r + ncta]) for r in range(0, cout, ncta)])
-                img_d = torch.as_tensor(img).to(dev)
-                bias_d = torch.as_tensor(bias).to(dev)
-                y = alloc(B * h * w * cout)
-                d.n, d.hw, d.cout, d.mid, d.cr, d.strips = B, h * w, cout, c, gw1.shape[0], strips
-                for i in range(4):
-                    d.tails[i] = xs[i].data_ptr()
-                d.gap_part = gap.data_ptr()
-                d.gw1, d.gb1, d.gw2, d.gb2 = (t_.data_ptr() for t_ in (gw1, gb1, gw2, gb2))
-                d.wimg, d.bias, d.out = img_d.data_ptr(), bias_d.data_ptr(), y.data_ptr()
-                d.gate_scratch = self.gate_tmp.data_ptr()
-                self._keep += [d, img_d, bias_d]
-                self._add('fm_osb_merge', C.byref(d))
-                self.n_tc += 1
-                self.n_merge = getattr(self, 'n_merge', 0) + 1
-                self.layer_bytes += 2 * (B * h * w * (4 * c + 2 * cout))
-                # bookkeeping of the skipped ops' reads
-                for kk in range(k, last_k + 1):
-                    for nm in self._reads(self.ops[kk]):
-                        if last.get(nm) == kk:
-                            release(nm)
-                if add_op[3] in live:
-                    release(add_op[3])
-                live[add_op[3]] = (y, cout, h, w)
-                trace('G', range(k, last_k + 1), list(srcs) + [srcs[0] + '.gap', ds_op[8] if ds_op else ident_name],
-                      [nhwc(add_op[3])])
-                skip_until = last_k
-                continue
-            elif kind == 'gate4':
-                _, name, c, srcs, acc = op
-                xs = [live[s_][0] for s_ in srcs]
-                _, xc, h, w = live[srcs[0]]
-                w1, b1, w2, b2 = dparam(name)
-                a = alloc(B * h * w * c)
-                if srcs[0] in pooled_by_tail:      # channel sums already produced by fm_osb_streams
-                    gap, strips = pooled_by_tail[srcs[0]]
-                    self._add('fm_channel_gate4_pooled', ptr(xs[0]), ptr(xs[1]), ptr(xs[2]), ptr(xs[3]), ptr(gap),
-                              strips, ptr(self.gate_tmp), ptr(w1), ptr(b1), ptr(w2), ptr(b2), ptr(a), B, h * w, c,
-                              w1.shape[0])
-                    trace('gate4_pooled', (k,), list(srcs) + [srcs[0] + '.gap'], [View(acc, a, 'nhwc', c, h, w)])
-                else:
-                    self._add('fm_channel_gate4', ptr(xs[0]), ptr(xs[1]), ptr(xs[2]), ptr(xs[3]), ptr(self.pooled),
-                              ptr(self.gate_tmp), ptr(w1), ptr(b1), ptr(w2), ptr(b2), ptr(a), B, h * w, c,
-                              w1.shape[0])
-                    trace(kind, (k,), list(srcs), [View(acc, a, 'nhwc', c, h, w)])
-                new = (acc, (a, c, h, w))
-            elif kind == 'add_relu':
-                if k in fused_add:        # folded into the preceding conv's epilogue
-                    continue
-                a, ac, h, w = live[op[1]]
-                b = live[op[2]][0]
-                y = alloc(B * h * w * ac)
-                self._add('fm_add_act', ptr(a), ptr(b), ptr(y), B * h * w * ac, _ACT['relu'])
-                new = (op[3], (y, ac, h, w))
-                trace(kind, (k,), [op[1], op[2]], [View(new[0], new[1][0], 'nhwc', *new[1][1:])])
-            elif kind == 'gap':
-                x, xc, h, w = live[op[1]]
-                y = alloc(B * xc, torch.float32)
-                self._add('fm_global_avgpool', ptr(x), ptr(y), B, h * w, xc)
-                new = (op[2], (y, xc, 1, 1))
-                trace(kind, (k,), [op[1]], [View(op[2], y, 'f32', xc)])
-            elif kind == 'fc':
-                _, name, cin, cout, src, dst = op
-                x = live[src][0]
-                wd, bd = dparam(name)
-                self._add('fm_fc_norm', ptr(x), ptr(wd), ptr(bd), ptr(self.out), B, cin, cout, 1, 1)
-                trace(kind, (k,), [src], [View(dst, self.out, 'f32', cout)])
-                new = None
-            else:
-                raise NotImplementedError(kind)
-            for name in self._reads(op):
-                if last.get(name) == k and not (kind == 'gate' and name == op[4]):
-                    release(name)
-            if new is not None:
-                if new[0] in live:
-                    release(new[0])
-                live[new[0]] = new[1]
-                views[new[0]] = self.trace[-1].outs[0]
+        last = {name: k for k, op in enumerate(self.ops) for name in _reads(op)}
+        for g in plan:
+            # a group allocates its outputs before its inputs are released, so no launch writes into its own input
+            defs = self._EMIT[g.kind](self, g)
+            for k in g.ops:
+                for name in _reads(self.ops[k]):
+                    if last[name] == k and defs.get(name) is not self._live.get(name):   # not the in-place gate
+                        self._release(name)
+            for name, entry in defs.items():
+                if self._live.get(name) is not entry:
+                    self._release(name)     # the previous holder of a rebound name
+                    self._live[name] = entry
 
-    def _match_osblock(self, k):
-        """ops[k] = '<blk>.conv1'; returns (tail buffer names of the four streams, index of the gate4 op) when the next
-        twenty ops are the Lite-3x3 chains a.0, b.0, b.1, c.0 .. d.3 feeding that gate, else None."""
-        ops = self.ops
-        if k + 21 >= len(ops):
-            return None
-        x1 = ops[k][9]
-        mid = ops[k][3]
-        tails = []
-        i = k + 1
-        for s_ in range(4):
-            prev = x1
-            for j in range(s_ + 1):
-                pw, dw = ops[i], ops[i + 1]
-                if pw[0] != 'conv' or dw[0] != 'dw' or pw[2] != mid or pw[3] != mid or pw[4] != 1 or pw[7] != 'linear' \
-                        or pw[8] != prev or dw[4] != pw[9] or dw[2] != mid or dw[3] != 'relu':
-                    return None
-                prev = dw[5]
-                i += 2
-            tails.append(prev)
-        g = ops[i]
-        if g[0] != 'gate4' or tuple(g[3]) != tuple(tails) or ops[k][7] != 'relu':
-            return None
-        return tails, i
+    def _alloc(self, numel, dtype=torch.float16):
+        free = self._free.get((numel, dtype))
+        if free:
+            return free.pop()
+        t = torch.zeros(numel, dtype=dtype, device=self.dev)
+        self._bufs.append(t)
+        return t
 
-    def _match_merge(self, k):
-        """ops[k] = gate4 of an OSBlock; returns (downsample conv or None, conv3, add_relu, index of add_relu) when
-        the ops that follow are [downsample 1x1] conv3 1x1 (linear, reads the gate output) and add_relu."""
-        ops = self.ops
-        acc = ops[k][4]
-        i = k + 1
-        ds = None
-        if i < len(ops) and ops[i][0] == 'conv' and ops[i][8] != acc:      # a conv beside conv3: the downsample branch
-            ds = ops[i]
-            i += 1
-        if i + 1 >= len(ops):
-            return None
-        c3, add = ops[i], ops[i + 1]
-        if c3[0] != 'conv' or c3[4] != 1 or c3[7] != 'linear' or c3[8] != acc or add[0] != 'add_relu':
-            return None
-        if c3[9] not in (add[1], add[2]):
-            return None
-        other = add[2] if add[1] == c3[9] else add[1]
-        if ds is not None and (ds[4] != 1 or ds[7] != 'linear' or ds[9] != other or ds[2] % 64):
-            return None
-        return ds, c3, add, i + 1
+    def _release(self, name):
+        t = self._live.pop(name, None)
+        if t is not None and name != 'input':
+            self._free.setdefault((t[0].numel(), t[0].dtype), []).append(t[0])
 
-    @staticmethod
-    def _reads(op):
-        kind = op[0]
-        if kind == 'conv':
-            return [op[8]]
-        if kind == 'dw':
-            return [op[4]]
-        if kind in ('maxpool3s2', 'avgpool2', 'gap'):
-            return [op[1]]
-        if kind == 'gate':
-            return [op[3], op[4]]
-        if kind == 'gate4':
-            return list(op[3])
-        if kind == 'add_relu':
-            return [op[1], op[2]]
-        if kind == 'fc':
-            return [op[4]]
-        return []
+    def _param(self, name):
+        """The device copies of a layer's weights, uploaded once."""
+        if name not in self._params:
+            self._params[name] = tuple(torch.as_tensor(a).to(self.dev) for a in self.weights[name])
+        return self._params[name]
+
+    def _record(self, g, ins, outs):
+        """Appends the trace entry of group g: the names of the views it reads, the Views it writes."""
+        self.trace.append(TraceEntry(g.kind, g.ops, [self._views[name] for name in ins], outs))
+        self._views.update((v.name, v) for v in outs)
+
+    def _bind(self, g, ins, name, entry):
+        """Records g as writing entry = (tensor, c, h, w) NHWC under name; returns the group's definitions."""
+        self._record(g, ins, [View(name, entry[0], 'nhwc', *entry[1:])])
+        return {name: entry}
+
+    def _emit_stem(self, g):
+        from .packing import pack_b_sw64
+        w7, b7 = self.weights[self.ops[0][1]]                        # [64][7][7][3]
+        wk = np.zeros((64, 7, 8, 4), np.float32)
+        wk[:, :, 1:8, :3] = w7
+        img = torch.as_tensor(pack_b_sw64(wk.reshape(64, 224))).to(self.dev)
+        b_d = torch.as_tensor(np.ascontiguousarray(b7, np.float32)).to(self.dev)
+        c, h, w = g.shape
+        y = self._alloc(self.max_batch * c * h * w)
+        self._keep += [img, b_d]
+        self._add('fm_osnet_stem', ptr(self.inp), self.max_batch, ptr(img), ptr(b_d), ptr(y))
+        self.n_tc += 1
+        self.layer_bytes += 2 * (self.inp.numel() + y.numel())
+        return self._bind(g, ['input'], self.ops[1][2], (y, c, h, w))
+
+    def _emit_S(self, g):
+        from .packing import pack_b_sw128
+        k, B, dev = g.ops[0], self.max_batch, self.dev
+        op = self.ops[k]
+        x, xc, h, w = self._live[op[8]]
+        mid, strips, names = op[3], g.info['strips'], g.info['tails']
+        w1, b1 = self.weights[op[1]]
+        w1_img = torch.as_tensor(pack_b_sw128(w1.reshape(mid, xc))).to(dev)
+        b1_d = torch.as_tensor(np.ascontiguousarray(b1, np.float32)).to(dev)
+        pw_imgs, dw_blobs = [], []
+        for i in range(10):
+            pw_op, dw_op = self.ops[k + 1 + 2 * i], self.ops[k + 2 + 2 * i]
+            wp, bp = self.weights[pw_op[1]]
+            wd, bd = self.weights[dw_op[1]]
+            pw_imgs.append(pack_b_sw128(wp.reshape(mid, mid)))
+            dw_blobs.append(np.concatenate([np.ascontiguousarray(wd, np.float32).astype(np.float16)
+                                            .reshape(-1).view(np.uint8),
+                                            np.ascontiguousarray(bp, np.float32).view(np.uint8),
+                                            np.ascontiguousarray(bd, np.float32).view(np.uint8)]))
+        pw_d = torch.as_tensor(np.concatenate(pw_imgs)).to(dev)
+        dw_d = torch.as_tensor(np.concatenate(dw_blobs)).to(dev)
+        tails = [self._alloc(B * h * w * mid) for _ in range(4)]
+        gap = torch.zeros(B * strips * 4 * mid, dtype=torch.float32, device=dev)
+        d = _lib.FmOsbStreams()
+        d.x, d.n, d.h, d.w, d.cin, d.mid = x.data_ptr(), B, h, w, xc, mid
+        d.w1, d.b1, d.pw, d.dw = w1_img.data_ptr(), b1_d.data_ptr(), pw_d.data_ptr(), dw_d.data_ptr()
+        for i in range(4):
+            d.tails[i] = tails[i].data_ptr()
+        d.gap_part = gap.data_ptr()
+        self._keep += [d, w1_img, b1_d, pw_d, dw_d, gap]
+        self._add('fm_osb_streams', C.byref(d))
+        self.n_tc += 1
+        self.n_osb += 1
+        self.layer_bytes += 2 * (B * h * w * (xc + 4 * mid))
+        # the strip sums: read by the G or gate4_pooled launch that follows, under the first tail's name + '.gap'
+        self._record(g, [op[8]], [View(tn, t, 'planar8', mid, h, w) for tn, t in zip(names, tails)]
+                     + [View(names[0] + '.gap', gap, 'gap_part', mid, h, w, strips=strips)])
+        return {tn: (t, mid, h, w) for tn, t in zip(names, tails)}
+
+    def _emit_G(self, g):
+        from .packing import pack_b_sw128
+        B, dev = self.max_batch, self.dev
+        _, name, c, srcs, acc = self.ops[g.ops[0]]
+        ds_op, c3_op, add_op, ncta = g.info['ds'], g.info['c3'], g.info['add'], g.info['ncta']
+        cout, h, w = g.shape
+        gap = self._views[srcs[0] + '.gap']
+        gw1, gb1, gw2, gb2 = self._param(name)
+        w3, b3 = self.weights[c3_op[1]]
+        wcat = w3.reshape(cout, c)
+        bias = np.asarray(b3, np.float32).copy()
+        ident_name = add_op[2] if add_op[1] == c3_op[9] else add_op[1]
+        d = _lib.FmOsbMerge()
+        if ds_op is not None:
+            wdn, bdn = self.weights[ds_op[1]]
+            cin = ds_op[2]
+            wcat = np.concatenate([wdn.reshape(cout, cin), wcat], 1)
+            bias += np.asarray(bdn, np.float32)
+            d.x, d.res, d.cin = self._live[ds_op[8]][0].data_ptr(), None, cin
+        else:
+            d.x, d.res, d.cin = None, self._live[ident_name][0].data_ptr(), cout
+        img = np.concatenate([pack_b_sw128(wcat[r:r + ncta]) for r in range(0, cout, ncta)])
+        img_d = torch.as_tensor(img).to(dev)
+        bias_d = torch.as_tensor(bias).to(dev)
+        y = self._alloc(B * h * w * cout)
+        d.n, d.hw, d.cout, d.mid, d.cr, d.strips = B, h * w, cout, c, gw1.shape[0], gap.strips
+        for i in range(4):
+            d.tails[i] = self._live[srcs[i]][0].data_ptr()
+        d.gap_part = gap.t.data_ptr()
+        d.gw1, d.gb1, d.gw2, d.gb2 = (t_.data_ptr() for t_ in (gw1, gb1, gw2, gb2))
+        d.wimg, d.bias, d.out = img_d.data_ptr(), bias_d.data_ptr(), y.data_ptr()
+        d.gate_scratch = self.gate_tmp.data_ptr()
+        self._keep += [d, img_d, bias_d]
+        self._add('fm_osb_merge', C.byref(d))
+        self.n_tc += 1
+        self.layer_bytes += 2 * (B * h * w * (4 * c + 2 * cout))
+        return self._bind(g, list(srcs) + [gap.name, ds_op[8] if ds_op else ident_name], add_op[3], (y, cout, h, w))
+
+    def _emit_conv(self, g):
+        """'conv', and 'conv+add': relu(conv(x) + residual) with the residual and the activation in the epilogue."""
+        _, name, cin, cout, ks, stride, pad, act, src, dst = self.ops[g.ops[0]]
+        B = self.max_batch
+        x, xc, h, w = self._live[src]
+        _, ho, wo = g.shape
+        wt, bs = self.weights[name]
+        if xc != cin:  # stem: physical 4 channels
+            wt = np.concatenate([wt, np.zeros(wt.shape[:3] + (xc - cin,), np.float32)], -1)
+        wd = torch.as_tensor(np.ascontiguousarray(wt)).to(self.dev).half().contiguous()
+        bd = torch.as_tensor(bs).to(self.dev).float().contiguous()
+        self._params[name] = (wd, bd)
+        y = self._alloc(B * ho * wo * cout)
+        if g.kind == 'conv':
+            self._conv(_conv_desc(B, h, w, xc, xc, 0, ho, wo, cout, cout, 0, ks, stride, pad, _ACT[act]), x, wd, bd, y)
+            return self._bind(g, [src], dst, (y, cout, ho, wo))
+        _, _, res, out = self.ops[g.ops[1]]
+        d = _conv_desc(B, h, w, xc, xc, 0, ho, wo, cout, cout, 0, ks, stride, pad, _ACT['relu'] | ACT_AFTER_RESIDUAL)
+        d.res_stride, d.res_offset = cout, 0
+        self._conv(d, x, wd, bd, y, residual=self._live[res][0])
+        return self._bind(g, [src, res], out, (y, cout, ho, wo))
+
+    def _emit_dw(self, g):
+        _, name, c, act, src, dst = self.ops[g.ops[0]]
+        B = self.max_batch
+        x, _, h, w = self._live[src]
+        wd, bd = self._param(name)
+        wd = wd.half().contiguous()
+        self._params[name] = (wd, bd)
+        y = self._alloc(B * h * w * c)
+        self._add('fm_dwconv3', ptr(x), ptr(wd), ptr(bd), ptr(y), B, h, w, c, _ACT[act])
+        self.layer_bytes += 2 * (2 * B * h * w * c + 9 * c)
+        return self._bind(g, [src], dst, (y, c, h, w))
+
+    def _emit_pool(self, g):
+        """'maxpool3s2' and 'avgpool2'."""
+        _, src, dst = self.ops[g.ops[0]]
+        B = self.max_batch
+        x, xc, h, w = self._live[src]
+        _, ho, wo = g.shape
+        y = self._alloc(B * ho * wo * xc)
+        if g.kind == 'maxpool3s2':
+            self._add('fm_maxpool_pad', ptr(x), ptr(y), B, h, w, xc, 3, 2, 1)
+        else:
+            self._add('fm_avgpool2', ptr(x), ptr(y), B, h, w, xc)
+        return self._bind(g, [src], dst, (y, xc, ho, wo))
+
+    def _emit_gate(self, g):
+        """acc (+)= src * gate(src), in place into acc once the first gate of a chain has allocated it."""
+        _, name, c, src, acc, accumulate = self.ops[g.ops[0]]
+        B = self.max_batch
+        x, _, h, w = self._live[src]
+        w1, b1, w2, b2 = self._param(name)
+        entry = self._live[acc] if acc in self._live else (self._alloc(B * h * w * c), c, h, w)
+        self._add('fm_channel_gate', ptr(x), ptr(self.pooled), ptr(self.gate_tmp), ptr(w1), ptr(b1), ptr(w2),
+                  ptr(b2), ptr(entry[0]), B, h * w, c, w1.shape[0], accumulate)
+        return self._bind(g, [src, acc] if accumulate else [src], acc, entry)
+
+    def _emit_gate4(self, g):
+        """'gate4', and 'gate4_pooled': the channel sums come from the S launch that wrote the four streams."""
+        _, name, c, srcs, acc = self.ops[g.ops[0]]
+        B = self.max_batch
+        xs = [ptr(self._live[s_][0]) for s_ in srcs]
+        _, h, w = g.shape
+        w1, b1, w2, b2 = self._param(name)
+        a = self._alloc(B * h * w * c)
+        if g.kind == 'gate4_pooled':
+            gap = self._views[srcs[0] + '.gap']
+            self._add('fm_channel_gate4_pooled', *xs, ptr(gap.t), gap.strips, ptr(self.gate_tmp), ptr(w1), ptr(b1),
+                      ptr(w2), ptr(b2), ptr(a), B, h * w, c, w1.shape[0])
+            return self._bind(g, list(srcs) + [gap.name], acc, (a, c, h, w))
+        self._add('fm_channel_gate4', *xs, ptr(self.pooled), ptr(self.gate_tmp), ptr(w1), ptr(b1), ptr(w2), ptr(b2),
+                  ptr(a), B, h * w, c, w1.shape[0])
+        return self._bind(g, list(srcs), acc, (a, c, h, w))
+
+    def _emit_add_relu(self, g):
+        _, a_name, b_name, dst = self.ops[g.ops[0]]
+        a, ac, h, w = self._live[a_name]
+        n = self.max_batch * h * w * ac
+        y = self._alloc(n)
+        self._add('fm_add_act', ptr(a), ptr(self._live[b_name][0]), ptr(y), n, _ACT['relu'])
+        return self._bind(g, [a_name, b_name], dst, (y, ac, h, w))
+
+    def _emit_gap(self, g):
+        _, src, dst = self.ops[g.ops[0]]
+        x, xc, h, w = self._live[src]
+        y = self._alloc(self.max_batch * xc, torch.float32)
+        self._add('fm_global_avgpool', ptr(x), ptr(y), self.max_batch, h * w, xc)
+        self._record(g, [src], [View(dst, y, 'f32', xc)])
+        return {dst: (y, xc, 1, 1)}
+
+    def _emit_fc(self, g):
+        """Writes the embeddings into self.out, which no later launch reads: defines no buffer."""
+        _, name, cin, cout, src, dst = self.ops[g.ops[0]]
+        wd, bd = self._param(name)
+        self._add('fm_fc_norm', ptr(self._live[src][0]), ptr(wd), ptr(bd), ptr(self.out), self.max_batch, cin, cout,
+                  1, 1)
+        self._record(g, [src], [View(dst, self.out, 'f32', cout)])
+        return {}
+
+    # group kind -> emitter: allocates the group's outputs, records its launch, trace entry and counters, and returns
+    # {name: (tensor, c, h, w)} of the buffers it defines
+    _EMIT = {'stem': _emit_stem, 'S': _emit_S, 'G': _emit_G, 'conv': _emit_conv, 'conv+add': _emit_conv,
+             'dw': _emit_dw, 'maxpool3s2': _emit_pool, 'avgpool2': _emit_pool, 'gate': _emit_gate,
+             'gate4': _emit_gate4, 'gate4_pooled': _emit_gate4, 'add_relu': _emit_add_relu, 'gap': _emit_gap,
+             'fc': _emit_fc}
 
     def load_nhwc8(self, x):
         """Copies crops given as [n][256][128][>= 3] fp16 (RGB first) into the engine's input buffer, whatever its

@@ -111,34 +111,50 @@ def synthetic_weights(ops, seed_base=5000, reduction=16, calibrate=True):
     return w
 
 
-def count_macs(ops, h=256, w=128):
-    """Multiply-accumulates per crop (dense convs + depthwise + fc)."""
-    shapes = {'input': (h, w)}
-    total = 0
+def infer_shapes(ops, h=256, w=128):
+    """The (c, h, w) of the tensor each op writes, in op order, for a 3-channel h x w input.  A list per op, not a
+    dict per name: an op list may bind a name twice (the stem writes 'x' with the conv and again with the pool)."""
+    named = {'input': (3, h, w)}
+    shapes = []
     for op in ops:
         kind = op[0]
         if kind == 'conv':
-            _, _, cin, cout, ks, stride, pad, _, src, dst = op
-            hh, ww = shapes[src]
-            ho, wo = (hh + 2 * pad - ks) // stride + 1, (ww + 2 * pad - ks) // stride + 1
-            shapes[dst] = (ho, wo)
-            total += cin * cout * ks * ks * ho * wo
+            _, _, _, cout, ks, stride, pad, _, src, dst = op
+            _, hh, ww = named[src]
+            shape = (cout, (hh + 2 * pad - ks) // stride + 1, (ww + 2 * pad - ks) // stride + 1)
         elif kind == 'dw':
-            _, _, c, _, src, dst = op
-            shapes[dst] = shapes[src]
-            total += 9 * c * shapes[src][0] * shapes[src][1]
+            shape, dst = (op[2],) + named[op[4]][1:], op[5]
         elif kind == 'maxpool3s2':
-            hh, ww = shapes[op[1]]
-            shapes[op[2]] = ((hh + 2 - 3) // 2 + 1, (ww + 2 - 3) // 2 + 1)
+            c, hh, ww = named[op[1]]
+            shape, dst = (c, (hh + 2 - 3) // 2 + 1, (ww + 2 - 3) // 2 + 1), op[2]
         elif kind == 'avgpool2':
-            hh, ww = shapes[op[1]]
-            shapes[op[2]] = (hh // 2, ww // 2)
+            c, hh, ww = named[op[1]]
+            shape, dst = (c, hh // 2, ww // 2), op[2]
         elif kind == 'gate':
-            shapes.setdefault(op[4], shapes[op[3]])
+            shape, dst = (op[2],) + named[op[3]][1:], op[4]
         elif kind == 'gate4':
-            shapes[op[4]] = shapes[op[3][0]]
+            shape, dst = (op[2],) + named[op[3][0]][1:], op[4]
         elif kind == 'add_relu':
-            shapes[op[3]] = shapes[op[1]]
+            shape, dst = named[op[1]], op[3]
+        elif kind == 'gap':
+            shape, dst = (named[op[1]][0], 1, 1), op[2]
         elif kind == 'fc':
+            shape, dst = (op[3], 1, 1), op[5]
+        else:
+            raise NotImplementedError(kind)
+        named[dst] = shape
+        shapes.append(shape)
+    return shapes
+
+
+def count_macs(ops, h=256, w=128):
+    """Multiply-accumulates per crop (dense convs + depthwise + fc)."""
+    total = 0
+    for op, (c, ho, wo) in zip(ops, infer_shapes(ops, h, w)):
+        if op[0] == 'conv':
+            total += op[2] * c * op[4] * op[4] * ho * wo
+        elif op[0] == 'dw':
+            total += 9 * c * ho * wo
+        elif op[0] == 'fc':
             total += op[2] * op[3]
     return total

@@ -110,6 +110,7 @@ def run_launch_by_launch(eng, crops, label):
     from oracle import nets64 as R
     n = eng.max_batch
     assert len(eng.trace) == len(eng.launches)
+    assert not eng._live, f"buffers still held after their last reader: {sorted(eng._live)}"
     eng.load_nhwc8(crops)
     last_read = {}
     for i, e in enumerate(eng.trace):
