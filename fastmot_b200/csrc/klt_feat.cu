@@ -645,7 +645,9 @@ __global__ void fast_score_kernel(const unsigned char* __restrict__ img, int w, 
 // Pixels are cut into 32-pixel words; warp w takes words w, w + 32, ... (lanes read consecutive pixels, four words'
 // scores are in flight at once), the keep decision of every pixel is taken once and kept as a ballot word in shared
 // memory; a block scan over the word popcounts gives every word its output offset, the scatter only replays bits.
-#define FAST_NMS_MAX_WORDS 4096      // 131 072 pixels at the background scale (1920x1080 x 0.1^2 = 20 736)
+// Images of more than FAST_NMS_MAX_WORDS words are walked in chunks of that many words, the output offset carried from
+// one chunk to the next (the default 1920x1080 x 0.1 background, 20 736 pixels, is one chunk).
+#define FAST_NMS_MAX_WORDS 4096
 __global__ void __launch_bounds__(1024) fast_nms_kernel(const unsigned char* __restrict__ score,
                                                          const unsigned char* __restrict__ mask, int w, int h,
                                                          float unscale_x, float unscale_y, float* __restrict__ out_pts,
@@ -656,79 +658,85 @@ __global__ void __launch_bounds__(1024) fast_nms_kernel(const unsigned char* __r
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const int n = w * h;
     const int words = (n + 31) >> 5;
-    for (int base = wid; base < words; base += 32 * 4) {
-        int sc[4];
+    int carry = 0;                                     // points of the chunks before this one
+    for (int c0 = 0; c0 < words; c0 += FAST_NMS_MAX_WORDS) {
+        const int cw = min(words - c0, FAST_NMS_MAX_WORDS);   // words of this chunk; s_* are indexed chunk-local
+        for (int base = wid; base < cw; base += 32 * 4) {
+            int sc[4];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            const int wd = base + 32 * u;
-            const int i = (wd << 5) + lane;
-            sc[u] = (wd < words && i < n) ? (int)score[i] : 0;
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            const int wd = base + 32 * u;              // warp-uniform
-            if (wd >= words) break;
-            const int i = (wd << 5) + lane;
-            bool ok = false;
-            if (sc[u] != 0) {
-                // a non-zero score is an interior pixel; neighbours outside [3, w-3) x [3, h-3) have score 0
-                const int v = sc[u];
-                ok = v > score[i - 1] && v > score[i + 1] && v > score[i - w - 1] && v > score[i - w] &&
-                     v > score[i - w + 1] && v > score[i + w - 1] && v > score[i + w] && v > score[i + w + 1] &&
-                     mask[i] != 0;
+            for (int u = 0; u < 4; ++u) {
+                const int lw = base + 32 * u;
+                const int i = ((c0 + lw) << 5) + lane;
+                sc[u] = (lw < cw && i < n) ? (int)score[i] : 0;
             }
-            const unsigned bal = __ballot_sync(0xffffffffu, ok);
-            if (lane == 0) s_bits[wd] = bal;
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                const int lw = base + 32 * u;              // warp-uniform
+                if (lw >= cw) break;
+                const int i = ((c0 + lw) << 5) + lane;
+                bool ok = false;
+                if (sc[u] != 0) {
+                    // a non-zero score is an interior pixel; neighbours outside [3, w-3) x [3, h-3) have score 0
+                    const int v = sc[u];
+                    ok = v > score[i - 1] && v > score[i + 1] && v > score[i - w - 1] && v > score[i - w] &&
+                         v > score[i - w + 1] && v > score[i + w - 1] && v > score[i + w] && v > score[i + w + 1] &&
+                         mask[i] != 0;
+                }
+                const unsigned bal = __ballot_sync(0xffffffffu, ok);
+                if (lane == 0) s_bits[lw] = bal;
+            }
         }
-    }
-    __syncthreads();
-    // exclusive prefix of the word popcounts: thread t owns words 4t .. 4t+3
-    int c[4], tot = 0;
+        __syncthreads();
+        // exclusive prefix of the word popcounts: thread t owns words 4t .. 4t+3
+        int c[4], tot = 0;
 #pragma unroll
-    for (int u = 0; u < 4; ++u) {
-        const int wd = 4 * tid + u;
-        c[u] = wd < words ? __popc(s_bits[wd]) : 0;
-        tot += c[u];
-    }
-    int v = tot;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int t = __shfl_up_sync(0xffffffffu, v, o);
-        if (lane >= o) v += t;
-    }
-    if (lane == 31) s_warp[wid] = v;
-    __syncthreads();
-    if (wid == 0) {
-        int t = s_warp[lane];
+        for (int u = 0; u < 4; ++u) {
+            const int lw = 4 * tid + u;
+            c[u] = lw < cw ? __popc(s_bits[lw]) : 0;
+            tot += c[u];
+        }
+        int v = tot;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) {
-            const int u = __shfl_up_sync(0xffffffffu, t, o);
-            if (lane >= o) t += u;
+            const int t = __shfl_up_sync(0xffffffffu, v, o);
+            if (lane >= o) v += t;
         }
-        s_warp[lane] = t;
-        if (lane == 31) *out_count = min(t, max_pts);
-    }
-    __syncthreads();
-    int run = v - tot + (wid ? s_warp[wid - 1] : 0);
+        if (lane == 31) s_warp[wid] = v;
+        __syncthreads();
+        if (wid == 0) {
+            int t = s_warp[lane];
 #pragma unroll
-    for (int u = 0; u < 4; ++u) {
-        const int wd = 4 * tid + u;
-        if (wd < words) s_pref[wd] = run;
-        run += c[u];
-    }
-    __syncthreads();
-    for (int wd = wid; wd < words; wd += 32) {
-        const unsigned bal = s_bits[wd];
-        if ((bal >> lane) & 1u) {
-            const int pos = s_pref[wd] + __popc(bal & ((1u << lane) - 1u));
-            if (pos < max_pts) {
-                const int i = (wd << 5) + lane;
-                const int y = i / w, x = i - y * w;
-                out_pts[2 * pos] = (float)x * unscale_x;      // _unscale_pts (flow.py:335-344)
-                out_pts[2 * pos + 1] = (float)y * unscale_y;
+            for (int o = 1; o < 32; o <<= 1) {
+                const int u = __shfl_up_sync(0xffffffffu, t, o);
+                if (lane >= o) t += u;
+            }
+            s_warp[lane] = t;
+        }
+        __syncthreads();
+        int run = carry + v - tot + (wid ? s_warp[wid - 1] : 0);
+#pragma unroll
+        for (int u = 0; u < 4; ++u) {
+            const int lw = 4 * tid + u;
+            if (lw < cw) s_pref[lw] = run;
+            run += c[u];
+        }
+        carry += s_warp[31];
+        __syncthreads();
+        for (int lw = wid; lw < cw; lw += 32) {
+            const unsigned bal = s_bits[lw];
+            if ((bal >> lane) & 1u) {
+                const int pos = s_pref[lw] + __popc(bal & ((1u << lane) - 1u));
+                if (pos < max_pts) {
+                    const int i = ((c0 + lw) << 5) + lane;
+                    const int y = i / w, x = i - y * w;
+                    out_pts[2 * pos] = (float)x * unscale_x;      // _unscale_pts (flow.py:335-344)
+                    out_pts[2 * pos + 1] = (float)y * unscale_y;
+                }
             }
         }
+        __syncthreads();                               // the next chunk rewrites s_bits, s_pref and s_warp
     }
+    if (tid == 0) *out_count = min(carry, max_pts);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -749,11 +757,13 @@ __global__ void __launch_bounds__(1024) gather_points_kernel(const float* __rest
     __syncthreads();
     if (tid == 0) {
         int acc = 0;
+        // begins are clamped to max_pts so that an overflowing frame (meta[3]) never makes the per-track kernels read
+        // past all_pts
         for (int k = 0; k < n_trk; ++k) {
-            trk_begin[k] = acc;
+            trk_begin[k] = min(acc, max_pts);
             acc += k < 2048 ? s_cnt[k] : min(kp_count[slots[k]], max_kp);
         }
-        trk_begin[n_trk] = acc;
+        trk_begin[n_trk] = min(acc, max_pts);
         int nb = *bg_count;
         if (acc + nb > max_pts) { meta[3] = 1; nb = max(0, max_pts - acc); acc = min(acc, max_pts); }
         meta[0] = acc;        // bg_begin = number of object points
@@ -835,9 +845,9 @@ extern "C" int fm_flow_keypoints_cfg(const unsigned char* prev_gray, int w, int 
 extern "C" int fm_fast_detect(const unsigned char* img, const unsigned char* mask, int w, int h, int threshold,
                               float unscale_x, float unscale_y, unsigned char* score, float* out_pts, int* out_count,
                               int max_pts, void* stream) {
+    FM_REQUIRE(threshold >= 0 && threshold <= 255, "fm_fast_detect: threshold must be in [0, 255]");
     cudaStream_t s = (cudaStream_t)stream;
     dim3 grid(fm_cdiv(w, 128), h);
-    FM_REQUIRE((long long)w * h <= 32ll * FAST_NMS_MAX_WORDS, "fm_fast_detect: image larger than 131072 pixels");
     fast_score_kernel<<<grid, 128, 0, s>>>(img, w, h, threshold, score);
     fast_nms_kernel<<<1, 1024, 0, s>>>(score, mask, w, h, unscale_x, unscale_y, out_pts, out_count, max_pts);
     FM_CHECK_LAUNCH("fm_fast_detect");

@@ -1,6 +1,6 @@
 // KLT image pyramid kernels (byte work, HBM/L2-bound): BGR->gray + 0.5x box mean in one pass, BGR->gray + an
 // INTER_LINEAR resize to any optical-flow size (both also reading YUV and BGRx frames in place, pixel_src.cuh),
-// 5-tap Gaussian pyrDown, int16 Scharr derivatives, 0.1x background image + mask.
+// 5-tap Gaussian pyrDown, int16 Scharr derivatives, background-scale image + mask.
 //
 // Reference: fastmot/flow.py:121-133, 153-154, 187-189 (cv2.cvtColor / cv2.resize) and the pyramid that
 // cv2.calcOpticalFlowPyrLK builds internally (flow.py:203-207; OpenCV lkpyramid.cpp: buildOpticalFlowPyramid,
@@ -131,30 +131,23 @@ __global__ void __launch_bounds__(256) scharr_kernel(const unsigned char* __rest
     deriv[(size_t)y * w + x] = make_short2((short)(s_p - s_m), (short)((d_p + d_m) * 3 + d_c * 10));
 }
 
-// 0.1x background image (cv2.resize INTER_LINEAR at 1/10: mean of the 2x2 block at (10x+4, 10y+4)) and
-// nearest-neighbour mask (src pixel (10x, 10y)); mask source is the owner map (>= NO_OWNER means foreground-free).
+// Background image (cv2.resize INTER_LINEAR, cv_linear.cuh) and its mask, cv2.resize INTER_NEAREST of the owner map
+// (FM_NO_OWNER is background, 255).  scale_x / scale_y are OpenCV's 1 / (dsize / ssize); INTER_NEAREST samples source
+// index floor(d * scale), which differs from floor(d * ssize / dsize) wherever the exact product is an integer.
 __global__ void bg_small_kernel(const unsigned char* __restrict__ gray, const int* __restrict__ owner, int w, int h,
                                 unsigned char* __restrict__ bg, unsigned char* __restrict__ bg_mask, int bw, int bh,
-                                double inv_sx, double inv_sy) {
+                                double scale_x, double scale_y) {
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
     const int y = blockIdx.y;
     if (x >= bw || y >= bh) return;
-    // generic cv2 INTER_LINEAR 8-bit fixed point (2048-scale coefficients), exact 2x2 mean when scale = 10
-    float fx = (float)((x + 0.5) * inv_sx - 0.5), fy = (float)((y + 0.5) * inv_sy - 0.5);
-    int sx = (int)floorf(fx), sy = (int)floorf(fy);
-    fx -= sx; fy -= sy;
-    if (sx < 0) { fx = 0; sx = 0; }
-    if (sx >= w - 1) { fx = 0; sx = w - 1; }
-    if (sy < 0) { fy = 0; sy = 0; }
-    if (sy >= h - 1) { fy = 0; sy = h - 1; }
-    const int a0 = (int)rintf((1.f - fx) * 2048.f), a1 = (int)rintf(fx * 2048.f);
-    const int b0 = (int)rintf((1.f - fy) * 2048.f), b1 = (int)rintf(fy * 2048.f);
-    const int sx1 = min(sx + 1, w - 1), sy1 = min(sy + 1, h - 1);
-    const unsigned char* r0 = gray + (size_t)sy * w;
-    const unsigned char* r1 = gray + (size_t)sy1 * w;
-    const int h0 = r0[sx] * a0 + r0[sx1] * a1, h1 = r1[sx] * a0 + r1[sx1] * a1;
-    bg[(size_t)y * bw + x] = (((b0 * (h0 >> 4)) >> 16) + ((b1 * (h1 >> 4)) >> 16) + 2) >> 2;
-    const int nx = min((int)floor(x * inv_sx), w - 1), ny = min((int)floor(y * inv_sy), h - 1);
+    const FmLinearTap c = fm_linear_col(x, scale_x, w), r = fm_linear_row(y, scale_y, h);
+    const unsigned char* r0 = gray + (size_t)r.i0 * w;
+    const unsigned char* r1 = gray + (size_t)r.i1 * w;
+    const int h0 = r0[c.i0] * c.w0 + r0[c.i1] * c.w1, h1 = r1[c.i0] * c.w0 + r1[c.i1] * c.w1;
+    bg[(size_t)y * bw + x] = fm_linear_v(r, h0, h1);
+    // clamps as selects (VIMNMX3, cv_linear.cuh)
+    const int nx0 = (int)floor(x * scale_x), ny0 = (int)floor(y * scale_y);
+    const int nx = nx0 < w - 1 ? nx0 : w - 1, ny = ny0 < h - 1 ? ny0 : h - 1;
     bg_mask[(size_t)y * bw + x] = owner[(size_t)ny * w + nx] == FM_NO_OWNER ? 255 : 0;
 }
 
@@ -208,7 +201,7 @@ extern "C" int fm_bg_small(const unsigned char* gray, const int* owner, int w, i
                            unsigned char* bg_mask, int bw, int bh, void* stream) {
     dim3 grid(fm_cdiv(bw, 128), bh);
     bg_small_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(gray, owner, w, h, bg, bg_mask, bw, bh,
-                                                            (double)w / bw, (double)h / bh);
+                                                            1.0 / ((double)bw / w), 1.0 / ((double)bh / h));
     FM_CHECK_LAUNCH("fm_bg_small");
     return FM_OK;
 }

@@ -27,6 +27,12 @@ GFTT_MAX_CAND = 4096
 _GFTT_KEYS = {"maxCorners", "qualityLevel", "blockSize", "useHarrisDetector", "k", "gradientSize"}
 
 
+def fast_corner_bound(w, h):
+    """Most corners FAST with non-max suppression can keep in a w x h image: the interior is (w-6) x (h-6) and no two
+    kept corners are 8-neighbours."""
+    return -(-max(w - 6, 0) // 2) * -(-max(h - 6, 0) // 2)
+
+
 def _depth_key(track):
     """Sort key equivalent to Track.__lt__ (fastmot/track.py:160-162): bottom edge, then younger first."""
     return (float(track.bboxes[-1][3]), -track.age)
@@ -67,6 +73,10 @@ class Flow:
         assert inlier_thresh >= 1
         self.inlier_thresh = inlier_thresh
         assert bg_feat_thresh >= 0
+        if bg_feat_thresh > 255:
+            # cv2's FAST tests most columns with the threshold cut to 8 bits and the last few with it clamped to 255,
+            # so above 255 its corners depend on where they lie in the image: no result to be exact against
+            raise ValueError(f"bg_feat_thresh must be at most 255 (the largest pixel contrast), got {bg_feat_thresh}")
         self.bg_feat_thresh = bg_feat_thresh
 
         self.obj_feat_params = {"maxCorners": 1000, "qualityLevel": 0.06, "blockSize": 3}
@@ -138,6 +148,9 @@ class Flow:
         self.bg = torch.zeros(bh, bw, dtype=u8, device=dev)
         self.bg_mask = torch.zeros(bh, bw, dtype=u8, device=dev)
         self.bg_score = torch.zeros(bh, bw, dtype=u8, device=dev)
+        # FAST's non-max suppression keeps no two touching corners, so the background buffers are sized to hold every
+        # corner the image can have and the point list is never cut short
+        max_bg_points = max(max_bg_points, fast_corner_bound(bw, bh))
         self.max_points, self.max_bg, self.max_tracks = max_points, max_bg_points, max_tracks
         self.bg_pts = torch.zeros(max_bg_points, 2, dtype=f32, device=dev)
         self.bg_count = torch.zeros(1, dtype=i32, device=dev)
@@ -147,11 +160,12 @@ class Flow:
         self.err = torch.zeros(max_points, dtype=f32, device=dev)
         self.trk_begin = torch.zeros(max_tracks + 1, dtype=i32, device=dev)
         self.slots_dev = torch.zeros(max_tracks, dtype=i32, device=dev)
-        self.meta = torch.zeros(4, dtype=i32, device=dev)
         self.jobs = torch.zeros(max_tracks * C.sizeof(_lib.FmTrackJob), dtype=u8, device=dev)
         self.scratch = torch.zeros(scratch_floats, dtype=f32, device=dev)
         self.scratch_cap = scratch_floats
-        self.flags = torch.zeros(32, dtype=i32, device=dev)   # [0] scratch counter, [1] kp status, [8:24] round flags
+        # [0] scratch counter, [1] kp status, [8:24] round flags, [24:28] gather meta (read back with the flags)
+        self.flags = torch.zeros(32, dtype=i32, device=dev)
+        self.meta = self.flags[24:28]
         self.good_idx = torch.zeros(max_bg_points, dtype=i32, device=dev)
         self.inl_idx = torch.zeros(max_bg_points, dtype=i32, device=dev)
         self.bg_kp = torch.zeros(max_bg_points, 2, dtype=f32, device=dev)
@@ -428,6 +442,9 @@ class Flow:
                               f"{GFTT_MAX_CAND} rows per track); set maxCorners between 1 and {GFTT_MAX_CAND}")
         if hf[1] != 0:
             raise MemoryError(f"Flow keypoint status code {int(hf[1])}")
+        if hf[27] != 0:
+            raise MemoryError("Flow point overflow: the track keypoints and background corners of this frame are more "
+                              f"than max_points={self.max_points}; raise max_points")
         return n == 0 or hf[8 + ((self.rounds_last - 1) & 15)] == 0 or self.rounds_last >= 2 * max(n, 1) + 2
 
     def finish_rounds(self, rounds=None):

@@ -408,12 +408,15 @@ int fm_flow_keypoints_cfg(const unsigned char* prev_gray, int w, int h, const do
                           int* scratch_counter, int* status, void* stream);
 
 /* cv2.FastFeatureDetector(threshold, nonmaxSuppression=True, TYPE_9_16).detect(img, mask) (flow.py:190) followed
- * by _unscale_pts (flow.py:335-344); output points in row-major order. score: w*h scratch bytes. */
+ * by _unscale_pts (flow.py:335-344); output points in row-major order, any image size, 0 <= threshold <= 255.
+ * score: w*h scratch bytes.
+ * At most max_pts points are written; no two corners touch, so max_pts >= ceil((w-6)/2) * ceil((h-6)/2) keeps all. */
 int fm_fast_detect(const unsigned char* img, const unsigned char* mask, int w, int h, int threshold, float unscale_x,
                    float unscale_y, unsigned char* score, float* out_pts, int* out_count, int max_pts, void* stream);
 
 /* flow.py:182-186, 199-200: all_prev_pts = concat(track keypoints) ++ background points.
- * trk_begin[n_trk + 1]; meta[0] = bg_begin, meta[1] = total points, meta[2] = #bg, meta[3] = overflow flag. */
+ * trk_begin[n_trk + 1]; meta[0] = bg_begin, meta[1] = total points, meta[2] = #bg, meta[3] = overflow flag (more
+ * than max_pts points: the list is cut at max_pts and every trk_begin is clamped to max_pts). */
 int fm_gather_points(const float* kp_pool, const int* kp_count, int max_kp, const int* slots, int n_trk,
                      const float* bg_pts, const int* bg_count, float* all_pts, int* trk_begin, int* meta,
                      int max_pts, void* stream);
